@@ -240,6 +240,24 @@ int rsb_class_histogram(const uint8_t* labels, int64_t n, int32_t C, uint64_t* c
  * -> uint8 [N][H*W] class indices, first maximum wins like np.argmax; C <= 255. */
 int rsb_head_argmax(const float* logits, uint8_t* mask, int32_t N, int32_t C, int32_t HW, void* stream);
 
+/* Test-time augmentation (no reference counterpart): average the class probabilities of up to 8 dihedral views of each tile.
+ * The views' inputs are made with rsb_augment_dihedral (square tiles) or rsb_augment_flip_rect (flips of any tile).
+ * logits fp32 [views*B][C][H][W], view-major (sample v*B + b is view v of tile b); ops_host: `views` ops in rsb_augment_dihedral's
+ * encoding (flip | k << 1), passed by value so the launch can be captured in a graph; odd k needs H == W. For every tile, class and
+ * pixel of the cropped output, the softmax over C of each view's logit at the pixel the op moved it to, as llrint(p * 2^59), is
+ * summed into acc int64 [B][C][H-2o][W-2o] (accumulate = 0 overwrites acc). Integer sums: the result does not depend on the order
+ * of the views or on how they are split over calls. C <= 255. */
+#define RSB_TTA_MAX_VIEWS 8
+int rsb_head_tta_accumulate(const float* logits, int64_t* acc, const int32_t* ops_host, int32_t views, int32_t B, int32_t C, int32_t H,
+                            int32_t W, int32_t overlap, int32_t accumulate, void* stream);
+/* 2-class acc [B][2][HW] summed over `views` views -> quant uint8 [B][HW]: np.digitize bins of the mean foreground probability
+ * (float)(acc[b][1] * 2^-59 / views), as rsb_head_quantize bins a single view */
+int rsb_head_tta_quantize(const int64_t* acc, uint8_t* quant, int32_t B, int32_t HW, int32_t views, void* stream);
+/* acc int64 [B][C][HW] -> uint8 [B][HW]: class of the largest sum (= largest mean probability), first maximum wins; C <= 255 */
+int rsb_head_tta_argmax(const int64_t* acc, uint8_t* mask, int32_t B, int32_t C, int32_t HW, void* stream);
+/* rsb_augment_dihedral's image transform for H x W tiles without a mask; when H != W only the flip bit of each op is used */
+int rsb_augment_flip_rect(const uint8_t* img, const int32_t* ops, uint8_t* out_img, int32_t N, int32_t H, int32_t W, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Host-side PNG codec for the files either side of the predict path (HOST pointers, plain C over zlib, no Python / GIL so the
  * tools' pool threads run truly in parallel). Pixel-identical to PIL; not a compute fallback -- no device work happens here.

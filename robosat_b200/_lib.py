@@ -140,6 +140,10 @@ SIGNATURES = {
     "rsb_softvote": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i64, _vp]),
     "rsb_class_histogram": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp]),
     "rsb_head_argmax": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "rsb_head_tta_accumulate": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(_i32), _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "rsb_head_tta_quantize": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "rsb_head_tta_argmax": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "rsb_augment_flip_rect": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_zlib_inflate": (ctypes.c_int, [ctypes.c_char_p, _i64, _vp, _i64]),
     "rsb_png_decode_rgb": (ctypes.c_int, [_vp, _i64, _vp, _i32, _i32]),
     "rsb_png_read_rgb": (ctypes.c_int, [ctypes.c_char_p, _vp, _i32, _i32]),

@@ -152,23 +152,23 @@ __global__ void maxpool_nhwc_split_kernel(const __half* __restrict__ src, int64_
 // Training-side augmentation on the device (robosat/transforms.py:127-221 as composed by train.py:253-258): per sample an optional
 // left-right flip followed by k counter-clockwise quarter turns (PIL's FLIP_LEFT_RIGHT / ROTATE_90), applied identically to the
 // RGB tile and its mask. op = flip | (k << 1). One thread per output pixel: 3 image bytes + 1 mask label (widened to int64, the
-// dtype the losses take -- MaskToTensor's job in the reference).
+// dtype the losses take -- MaskToTensor's job in the reference). Tiles are H x W; when H != W only the flip bit of an op is used.
 __global__ void augment_dihedral_kernel(const uint8_t* __restrict__ img, const uint8_t* __restrict__ mask, const int32_t* __restrict__ ops,
-                                        uint8_t* __restrict__ out_img, int64_t* __restrict__ out_mask, int N, int S) {
-    const int64_t total = static_cast<int64_t>(N) * S * S;
+                                        uint8_t* __restrict__ out_img, int64_t* __restrict__ out_mask, int N, int H, int W) {
+    const int64_t total = static_cast<int64_t>(N) * H * W;
     for (int64_t gid = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; gid < total; gid += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int x = static_cast<int>(gid % S);
-        const int y = static_cast<int>((gid / S) % S);
-        const int n = static_cast<int>(gid / (static_cast<int64_t>(S) * S));
-        const int op = ops[n];
+        const int x = static_cast<int>(gid % W);
+        const int y = static_cast<int>((gid / W) % H);
+        const int n = static_cast<int>(gid / (static_cast<int64_t>(H) * W));
+        const int op = ops[n] & (H == W ? 7 : 1);  // a non-square tile can only be flipped
         int sy = y, sx = x;
         for (int k = (op >> 1) & 3; k > 0; --k) {  // undo the quarter turns: ROTATE_90 writes out[y][x] = in[x][S-1-y]
             const int t = sy;
             sy = sx;
-            sx = S - 1 - t;
+            sx = W - 1 - t;
         }
-        if (op & 1) sx = S - 1 - sx;               // undo the flip: out[y][x] = in[y][S-1-x]
-        const int64_t src = (static_cast<int64_t>(n) * S + sy) * S + sx;
+        if (op & 1) sx = W - 1 - sx;               // undo the flip: out[y][x] = in[y][W-1-x]
+        const int64_t src = (static_cast<int64_t>(n) * H + sy) * W + sx;
         const uint8_t* s3 = img + src * 3;
         uint8_t* d3 = out_img + gid * 3;
         d3[0] = s3[0];
@@ -210,6 +210,113 @@ __global__ void head_quantize_kernel(const float* __restrict__ logits, uint8_t* 
     const float pfg = e1 / (e0 + e1);
     if (probs_fg) probs_fg[gid] = pfg;
     quant[gid] = static_cast<uint8_t>(digitize256(pfg));  // 256 wraps to 0 exactly like .astype(np.uint8)
+}
+
+// Test-time augmentation head. View v of tile b is logits sample v*B + b, computed from the tile transformed by op v
+// (rsb_augment_dihedral's encoding), so pixel p of the tile's cropped output sits at forward(op, p) in that view. Probabilities
+// are summed as int64 fixed point (one = 2^59): integer addition is associative, so the sum is the same bit for bit whatever
+// the order of the views and however they are split over calls.
+constexpr double kTtaOne = 576460752303423488.0;  // 2^59
+
+struct TtaOps {
+    int32_t op[RSB_TTA_MAX_VIEWS];
+};
+
+// where pixel (y, x) of an OH x OW crop lies after a left-right flip (op & 1) and k = op >> 1 counter-clockwise quarter turns.
+// The crop is centred, so this is also the map of the whole tile restricted to it. Odd k needs OH == OW.
+__device__ __forceinline__ void tta_forward_map(int op, int OH, int OW, int y, int x, int& vy, int& vx) {
+    if (op & 1) x = OW - 1 - x;
+    switch ((op >> 1) & 3) {
+        case 0: vy = y; vx = x; break;
+        case 1: vy = OW - 1 - x; vx = y; break;   // ROTATE_90: out[y][x] = in[x][S-1-y]
+        case 2: vy = OH - 1 - y; vx = OW - 1 - x; break;
+        default: vy = x; vx = OH - 1 - y; break;
+    }
+}
+
+// One block per TW x TW window of one tile's cropped output. Per view, the block stages the matching TW x TW window of the view's
+// logits (all C classes) in shared memory with row-contiguous global reads, so the transposed views read HBM as coalesced as the
+// identity view; the padded pitch keeps the transposed shared-memory reads free of bank conflicts. Each thread keeps the sums of
+// its own pixels in shared memory across the views and writes them once.
+__global__ void head_tta_accumulate_kernel(const float* __restrict__ logits, int64_t* __restrict__ acc, TtaOps ops, int V, int B, int C,
+                                           int H, int W, int o, int TW, int accumulate) {
+    extern __shared__ __align__(16) unsigned char tta_smem[];
+    const int OH = H - 2 * o, OW = W - 2 * o;
+    const int pitch = TW + 1, npix = TW * TW;
+    int64_t* sum = reinterpret_cast<int64_t*>(tta_smem);     // [C][TW * TW]
+    float* win = reinterpret_cast<float*>(sum + C * npix);    // [C][TW][TW + 1]
+    const int b = blockIdx.z, Y0 = blockIdx.y * TW, X0 = blockIdx.x * TW;
+    const int64_t hw = static_cast<int64_t>(H) * W;
+    const int cstride = TW * pitch;
+    for (int v = 0; v < V; ++v) {
+        const int op = ops.op[v];
+        int ay, ax, by, bx;  // the view window is the box spanned by the images of the output window's corners
+        tta_forward_map(op, OH, OW, Y0, X0, ay, ax);
+        tta_forward_map(op, OH, OW, Y0 + TW - 1, X0 + TW - 1, by, bx);
+        const int vy0 = min(ay, by), vx0 = min(ax, bx);
+        const float* src = logits + static_cast<int64_t>(v * B + b) * C * hw;
+        for (int i = threadIdx.x; i < C * npix; i += blockDim.x) {
+            const int c = i / npix, r = (i / TW) % TW, col = i % TW;
+            const int vy = vy0 + r, vx = vx0 + col;
+            if (vy >= 0 && vy < OH && vx >= 0 && vx < OW) win[c * cstride + r * pitch + col] = src[c * hw + static_cast<int64_t>(vy + o) * W + (vx + o)];
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < npix; i += blockDim.x) {
+            const int y = Y0 + i / TW, x = X0 + i % TW;
+            if (y >= OH || x >= OW) continue;
+            int vy, vx;
+            tta_forward_map(op, OH, OW, y, x, vy, vx);
+            const float* l = win + (vy - vy0) * pitch + (vx - vx0);
+            // softmax as head_quantize_kernel / softmax_nchw_kernel compute it (max-subtracted expf; for C = 2, e1 / (e0 + e1))
+            float m = l[0];
+            for (int c = 1; c < C; ++c) m = fmaxf(m, l[c * cstride]);
+            float s = 0.f;
+            for (int c = 0; c < C; ++c) s += expf(l[c * cstride] - m);
+            for (int c = 0; c < C; ++c) {
+                const int64_t q = llrint(static_cast<double>(expf(l[c * cstride] - m) / s) * kTtaOne);
+                int64_t& a = sum[c * npix + i];
+                a = v == 0 ? q : a + q;
+            }
+        }
+        __syncthreads();
+    }
+    for (int i = threadIdx.x; i < npix; i += blockDim.x) {
+        const int y = Y0 + i / TW, x = X0 + i % TW;
+        if (y >= OH || x >= OW) continue;
+        for (int c = 0; c < C; ++c) {
+            int64_t* d = acc + (static_cast<int64_t>(b * C + c) * OH + y) * OW + x;
+            *d = accumulate ? *d + sum[c * npix + i] : sum[c * npix + i];
+        }
+    }
+}
+
+// mean foreground probability of `views` summed views (class 1 of a 2-class acc [N][2][HW]) -> np.digitize bins
+__global__ void head_tta_quantize_kernel(const int64_t* __restrict__ acc, uint8_t* __restrict__ quant, int N, int64_t HW, int views) {
+    const int64_t total = static_cast<int64_t>(N) * HW;
+    const int64_t gid = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (gid >= total) return;
+    const int64_t n = gid / HW, pix = gid % HW;
+    const float pfg = static_cast<float>(static_cast<double>(acc[(n * 2 + 1) * HW + pix]) * (1.0 / kTtaOne) / views);
+    quant[gid] = static_cast<uint8_t>(digitize256(pfg));
+}
+
+// class index of the largest summed probability (the largest mean), first maximum wins like np.argmax
+__global__ void head_tta_argmax_kernel(const int64_t* __restrict__ acc, uint8_t* __restrict__ mask, int N, int C, int64_t HW) {
+    const int64_t total = static_cast<int64_t>(N) * HW;
+    const int64_t gid = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (gid >= total) return;
+    const int64_t n = gid / HW, pix = gid % HW;
+    const int64_t* a = acc + n * C * HW + pix;
+    int64_t m = a[0];
+    int best = 0;
+    for (int c = 1; c < C; ++c) {
+        const int64_t v = a[c * HW];
+        if (v > m) {
+            m = v;
+            best = c;
+        }
+    }
+    mask[gid] = static_cast<uint8_t>(best);
 }
 
 // Halo stitch (robosat/tiles.py:162-227 `buffer_tile_image`): canvas pixel (Y, X) of the (S+2o)^2 buffered tile comes from the
@@ -417,9 +524,59 @@ extern "C" int rsb_augment_dihedral(const uint8_t* img, const uint8_t* mask, con
     if (!img || !ops || !out_img || N <= 0 || S <= 0 || (mask && !out_mask)) return set_error(RSB_E_INVALID, "augment_dihedral: bad arguments");
     if (img == out_img) return set_error(RSB_E_INVALID, "augment_dihedral: cannot run in place");
     const int64_t total = static_cast<int64_t>(N) * S * S;
-    augment_dihedral_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(img, mask, ops, out_img, out_mask, N, S);
+    augment_dihedral_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(img, mask, ops, out_img, out_mask, N, S, S);
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "augment_dihedral launch");
+}
+
+extern "C" int rsb_augment_flip_rect(const uint8_t* img, const int32_t* ops, uint8_t* out_img, int32_t N, int32_t H, int32_t W, void* stream) {
+    if (!img || !ops || !out_img || N <= 0 || H <= 0 || W <= 0) return set_error(RSB_E_INVALID, "augment_flip_rect: bad arguments");
+    if (img == out_img) return set_error(RSB_E_INVALID, "augment_flip_rect: cannot run in place");
+    const int64_t total = static_cast<int64_t>(N) * H * W;
+    augment_dihedral_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(img, nullptr, ops, out_img, nullptr, N, H, W);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "augment_flip_rect launch");
+}
+
+// bytes of dynamic shared memory of head_tta_accumulate_kernel for a TW x TW window of C classes
+static inline int tta_smem_bytes(int C, int TW) { return C * TW * TW * 8 + C * TW * (TW + 1) * 4; }
+
+extern "C" int rsb_head_tta_accumulate(const float* logits, int64_t* acc, const int32_t* ops_host, int32_t views, int32_t B, int32_t C, int32_t H,
+                                       int32_t W, int32_t overlap, int32_t accumulate, void* stream) {
+    if (!logits || !acc || !ops_host || views < 1 || views > RSB_TTA_MAX_VIEWS || B <= 0 || C < 1 || C > 255 || overlap < 0 ||
+        H - 2 * overlap <= 0 || W - 2 * overlap <= 0 || (accumulate != 0 && accumulate != 1))
+        return set_error(RSB_E_INVALID, "head_tta_accumulate: bad arguments");
+    TtaOps ops = {};
+    for (int v = 0; v < views; ++v) {
+        if (ops_host[v] < 0 || ops_host[v] > 7) return set_error(RSB_E_INVALID, "head_tta_accumulate: ops must be in 0..7");
+        if (H != W && ((ops_host[v] >> 1) & 1)) return set_error(RSB_E_INVALID, "head_tta_accumulate: quarter turns need a square tile");
+        ops.op[v] = ops_host[v];
+    }
+    // the widest window whose staging fits the default 48 KB of shared memory (32 x 32 up to C = 3)
+    int TW = 32;
+    while (TW > 1 && tta_smem_bytes(C, TW) > 48 * 1024) TW /= 2;
+    const int OH = H - 2 * overlap, OW = W - 2 * overlap;
+    const dim3 grid((OW + TW - 1) / TW, (OH + TW - 1) / TW, B);
+    head_tta_accumulate_kernel<<<grid, 256, tta_smem_bytes(C, TW), static_cast<cudaStream_t>(stream)>>>(logits, acc, ops, views, B, C, H, W, overlap,
+                                                                                                         TW, accumulate);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "head_tta_accumulate launch");
+}
+
+extern "C" int rsb_head_tta_quantize(const int64_t* acc, uint8_t* quant, int32_t B, int32_t HW, int32_t views, void* stream) {
+    if (!acc || !quant || B <= 0 || HW <= 0 || views < 1) return set_error(RSB_E_INVALID, "head_tta_quantize: bad arguments");
+    const int64_t total = static_cast<int64_t>(B) * HW;
+    head_tta_quantize_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(acc, quant, B, HW, views);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "head_tta_quantize launch");
+}
+
+extern "C" int rsb_head_tta_argmax(const int64_t* acc, uint8_t* mask, int32_t B, int32_t C, int32_t HW, void* stream) {
+    if (!acc || !mask || B <= 0 || C <= 0 || C > 255 || HW <= 0) return set_error(RSB_E_INVALID, "head_tta_argmax: bad arguments");
+    const int64_t total = static_cast<int64_t>(B) * HW;
+    head_tta_argmax_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(acc, mask, B, C, HW);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "head_tta_argmax launch");
 }
 
 extern "C" int rsb_head_quantize(const float* logits, uint8_t* quant, float* probs_fg, int32_t N, int32_t H, int32_t W,

@@ -12,18 +12,27 @@ import torch
 
 from robosat_b200 import _lib
 from robosat_b200.engine import UNetEngine
+from robosat_b200.tta import TtaChain
 
 
 class TilePredictor:
-    def __init__(self, state_dict, num_classes, batch, size, overlap=0, device="cuda", depth=2, precision=None, use_graph=False):
+    def __init__(self, state_dict, num_classes, batch, size, overlap=0, device="cuda", depth=2, precision=None, use_graph=False, tta="none"):
         """size: net input extent (tile_size + 2*overlap, predict.py:75); depth: in-flight batches for copy/compute overlap.
         use_graph=True captures the 60 launches of (network + head) once per slot into a CUDA graph and replays it: ONE driver
         call per batch instead of 60 ctypes launches. The kernels and results are identical; it matters when the launching thread
         shares the interpreter with decode / encode / consumer threads (`rs predict`: the 60 launches took 5 ms per batch there and
-        the device ran ahead of them). If capture fails the predictor keeps launching kernel by kernel (`graph_error` says why)."""
+        the device ran ahead of them). If capture fails the predictor keeps launching kernel by kernel (`graph_error` says why).
+        tta="flip" | "d4": the bins are those of the mean probability over 2 | 8 dihedral views of each tile (robosat_b200/tta.py);
+        the network then runs on an engine of B*V/P tiles, P passes per batch, and the graph records the whole chain."""
         self.device = torch.device(device)
         self.batch, self.size, self.overlap, self.classes = batch, size, overlap, num_classes
-        self.engine = UNetEngine(state_dict, num_classes, batch, size, size, device=self.device, precision=precision)
+        self.tta = None
+        if tta == "none":
+            self.engine = UNetEngine(state_dict, num_classes, batch, size, size, device=self.device, precision=precision)
+        else:
+            engine_batch = TtaChain.engine_batch(tta, batch)
+            self.engine = UNetEngine(state_dict, num_classes, engine_batch, size, size, device=self.device, precision=precision)
+            self.tta = TtaChain(self.engine, tta, batch, size, size, num_classes, overlap, device=self.device)
         self.out_size = size - 2 * overlap
         self.depth = depth
         self._slots = []
@@ -54,6 +63,12 @@ class TilePredictor:
         if g is not None:
             g.replay()
         else:
+            self._enqueue(slot)
+
+    def _enqueue(self, slot):
+        if self.tta is not None:
+            self.tta.quantize(slot["d_in"], slot["d_q"])
+        else:
             self.quantize(self.engine.forward(slot["d_in"]), slot["d_q"])
 
     def _capture_graphs(self):
@@ -63,14 +78,14 @@ class TilePredictor:
         with torch.cuda.stream(side):
             for slot in self._slots:
                 slot["d_in"].zero_()
-                self.quantize(self.engine.forward(slot["d_in"]), slot["d_q"])
+                self._enqueue(slot)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         try:
             for slot in self._slots:
                 graph = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(graph, capture_error_mode="thread_local"):
-                    self.quantize(self.engine.forward(slot["d_in"]), slot["d_q"])
+                    self._enqueue(slot)
                 slot["graph"] = graph
         except Exception as exc:  # same kernels, launched one by one
             self.graph_error = "%s: %s" % (type(exc).__name__, exc)
@@ -92,6 +107,8 @@ class TilePredictor:
         return out_u8
 
     def num_launches(self):
+        if self.tta is not None:
+            return self.tta.num_launches()
         return self.engine.num_launches() + 1
 
     # ------------------------------------------------------------------ host -> host

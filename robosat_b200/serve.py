@@ -16,6 +16,7 @@ import torch
 from PIL import Image
 
 from robosat_b200 import _lib
+from robosat_b200 import tta as tta_mod
 from robosat_b200.colors import make_palette
 from robosat_b200.engine import UNetEngine
 
@@ -23,11 +24,20 @@ from robosat_b200.engine import UNetEngine
 class SegmentEngine:
     """uint8 RGB tiles [B, H, W, 3] (host) -> uint8 class-index masks [B, H, W] (host), graph-replayed."""
 
-    def __init__(self, state_dict, num_classes, height, width, batch=1, device="cuda", use_graph=True, precision=None):
+    def __init__(self, state_dict, num_classes, height, width, batch=1, device="cuda", use_graph=True, precision=None, tta="none"):
+        """tta="flip" | "d4": the mask is the argmax of the mean probability over 2 | 8 dihedral views (robosat_b200/tta.py), all
+        of them in one engine of B*V tiles up to 32 (a batch-1 d4 request is one 8-tile forward). "d4" needs height == width."""
         assert num_classes <= 255
         self.device = torch.device(device)
         self.batch, self.H, self.W, self.classes = batch, height, width, num_classes
-        self.engine = UNetEngine(state_dict, num_classes, batch, height, width, device=self.device, precision=precision)
+        self.tta = None
+        if tta == "none":
+            self.engine = UNetEngine(state_dict, num_classes, batch, height, width, device=self.device, precision=precision)
+        else:
+            tta_mod.check_shape(tta, height, width)
+            engine_batch = tta_mod.TtaChain.engine_batch(tta, batch)
+            self.engine = UNetEngine(state_dict, num_classes, engine_batch, height, width, device=self.device, precision=precision)
+            self.tta = tta_mod.TtaChain(self.engine, tta, batch, height, width, num_classes, device=self.device)
         self.h_in = torch.empty((batch, height, width, 3), dtype=torch.uint8, pin_memory=True)
         self.d_in = torch.empty((batch, height, width, 3), dtype=torch.uint8, device=self.device)
         self.d_mask = torch.empty((batch, height, width), dtype=torch.uint8, device=self.device)
@@ -40,6 +50,10 @@ class SegmentEngine:
     def _enqueue(self):
         """H2D, forward, argmax, D2H on the current stream (also what the graph records)."""
         self.d_in.copy_(self.h_in, non_blocking=True)
+        if self.tta is not None:
+            self.tta.argmax(self.d_in, self.d_mask)
+            self.h_mask.copy_(self.d_mask, non_blocking=True)
+            return
         logits = self.engine.forward(self.d_in)
         _lib.check(_lib.load().rsb_head_argmax(logits.data_ptr(), self.d_mask.data_ptr(), self.batch, self.classes, self.H * self.W,
                                                _lib.current_stream_ptr()), "rsb_head_argmax")
@@ -89,7 +103,10 @@ class SegmentEngine:
 class Predictor:
     """Same constructor and `segment(image) -> PIL.Image` contract as robosat/tools/serve.py:135-172."""
 
-    def __init__(self, checkpoint, model, dataset):
+    def __init__(self, checkpoint, model, dataset, tta="none"):
+        """tta: "none", "flip" or "d4" test-time augmentation of every request (SegmentEngine)"""
+        tta_mod.views(tta)  # an unknown mode fails here, not at the first request
+        self.tta = tta
         cuda = model["common"]["cuda"]
         assert torch.cuda.is_available() or not cuda, "cuda is available when requested"
         if not cuda:
@@ -108,7 +125,8 @@ class Predictor:
     def _engine_for(self, height, width):
         eng = self._engines.get((height, width))
         if eng is None:
-            eng = self._engines[(height, width)] = SegmentEngine(self.state_dict, self.num_classes, height, width, device=self.device)
+            eng = self._engines[(height, width)] = SegmentEngine(self.state_dict, self.num_classes, height, width, device=self.device,
+                                                                     tta=self.tta)
         return eng
 
     def segment(self, image):

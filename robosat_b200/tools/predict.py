@@ -35,6 +35,8 @@ def add_parser(subparser):
     parser.add_argument("probs", type=str, help="directory to save slippy map probability masks to")
     parser.add_argument("--model", type=str, required=True, help="path to model configuration file")
     parser.add_argument("--dataset", type=str, required=True, help="path to dataset configuration file")
+    parser.add_argument("--tta", type=str, default="none", choices=["none", "flip", "d4"],
+                        help="test-time augmentation: mean probability over flipped (flip) or all 8 dihedral (d4) views of each tile")
     parser.set_defaults(func=main)
 
 
@@ -104,6 +106,7 @@ def run_shard(rank, world, args, device, sd, num_classes, stats=None):
 
     t_start = time.perf_counter()
     st = stats if stats is not None else {}
+    tta = getattr(args, "tta", "none")  # Namespaces built by callers that predate the flag have no attribute
     size = args.tile_size + 2 * args.overlap
     palette = continuous_palette_for_color("pink", 256)
     # host cores of this rank -- min(affinity, cgroup CPU quota): the GPU boxes report 128 hardware threads under a quota of 16
@@ -145,7 +148,8 @@ def run_shard(rank, world, args, device, sd, num_classes, stats=None):
         lo, hi = shard_range(len(directory), rank, world)
         loader = DataLoader(Subset(directory, range(lo, hi)), batch_size=args.batch_size, num_workers=args.workers)
         predictor = TilePredictor(sd, num_classes, args.batch_size, size, overlap=args.overlap, device=device,
-                                   use_graph=os.environ.get("RSB_PREDICT_GRAPH", "1") == "1", depth=int(os.environ.get("RSB_PREDICT_DEPTH", "3")))
+                                   use_graph=os.environ.get("RSB_PREDICT_GRAPH", "1") == "1", depth=int(os.environ.get("RSB_PREDICT_DEPTH", "3")),
+                                   tta=tta)
         st.update(tiles=hi - lo, batches=len(loader), decode_wait_s=0.0)
         with ThreadPoolExecutor(max_workers=pool_threads) as pool:
             pending = []
@@ -179,7 +183,8 @@ def run_shard(rank, world, args, device, sd, num_classes, stats=None):
         cache = DeviceTileCache(index, args.tile_size, capacity, device=device, workers=decode_threads)
         stitcher = HaloStitcher(cache, args.overlap, args.batch_size)
         predictor = TilePredictor(sd, num_classes, args.batch_size, size, overlap=args.overlap, device=device,
-                                   use_graph=os.environ.get("RSB_PREDICT_GRAPH", "1") == "1", depth=int(os.environ.get("RSB_PREDICT_DEPTH", "3")))
+                                   use_graph=os.environ.get("RSB_PREDICT_GRAPH", "1") == "1", depth=int(os.environ.get("RSB_PREDICT_DEPTH", "3")),
+                                   tta=tta)
         chunks = [mine[i:i + args.batch_size] for i in range(0, len(mine), args.batch_size)]
         st.update(tiles=len(mine), batches=len(chunks), decode_threads=decode_threads)
         st["setup_s"] = time.perf_counter() - t_start  # enumerate + plan (weight folding / packing) + buffers, before the first batch

@@ -19,6 +19,8 @@ def add_parser(subparser):
     parser.add_argument("--tile_size", type=int, default=512, help="tile size for slippy map tiles")
     parser.add_argument("--host", type=str, default="127.0.0.1", help="host to serve on")
     parser.add_argument("--port", type=int, default=5000, help="port to serve on")
+    parser.add_argument("--tta", type=str, default="none", choices=["none", "flip", "d4"],
+                        help="test-time augmentation: argmax of the mean probability over flipped (flip) or all 8 dihedral (d4) views")
     parser.set_defaults(func=main)
 
 
@@ -72,6 +74,6 @@ def main(args):
         import requests
     except ImportError as exc:
         sys.exit("Error: rs serve needs flask and requests for its HTTP shell (%s)" % exc)
-    predictor = Predictor(args.checkpoint, model, dataset)
+    predictor = Predictor(args.checkpoint, model, dataset, tta=args.tta)
     app = make_app(predictor, args.url, token, args.tile_size, session=requests.Session())
     app.run(host=args.host, port=args.port, threaded=False)
