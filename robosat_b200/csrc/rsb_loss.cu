@@ -129,7 +129,10 @@ __global__ void focal_finish_kernel(const float* __restrict__ logits, const int6
         const float logp = (l[static_cast<int64_t>(t) * HW] - m) - logf(s);
         const float pt = expf(l[static_cast<int64_t>(t) * HW] - m) / s;
         const float q = 1.0f - pt;
-        const float k = powf(q, gamma) - gamma * powf(q, gamma - 1.0f) * pt * logp;
+        // gamma == 0: the penalty is the constant 1 and its derivative term is zero, as in torch's pow backward (exponent 0
+        // gives a zero gradient). Evaluated, it would be 0 * powf(0, -1) = 0 * inf = NaN wherever softmax saturates to p_t = 1.
+        const float dpen = gamma == 0.0f ? 0.0f : gamma * powf(q, gamma - 1.0f) * pt * logp;
+        const float k = powf(q, gamma) - dpen;
         const float w = -(weight ? weight[t] : 1.0f) * inv_den * k;
         for (int c = 0; c < C; ++c) {
             const float p = expf(l[c * HW] - m) / s;

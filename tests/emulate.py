@@ -60,25 +60,31 @@ def _pair(ptr, plane, shape, strides):
     return v
 
 
-def run_desc(d):
+def run_desc(d, sink=None):
     """Execute descriptor `d` (host pointers) and write its outputs like the device kernel would.
     Split descriptors: operands are hi + lo pairs; the contraction is done in float64 (the kernel's fp32 accumulation of
-    hi*hi + hi*lo + lo*hi differs from it by ~1e-7 relative), the epilogue in fp32 exactly like the kernel."""
+    hi*hi + hi*lo + lo*hi differs from it by ~1e-7 relative), the epilogue in fp32 exactly like the kernel.
+    sink (fast mode-0 descriptors only): float64 reference mode. Nothing is written; for every output phase
+    sink(ptr, shape, strides, value, magnitude) receives the exact float64 result (+ residual, ReLU) of the fp16 operands and
+    the same contraction over |x|*|w| (+ |residual|), which scales the accumulation error of the kernel."""
     split = bool(d.split)
+    f64 = sink is not None
+    assert not (f64 and (split or d.mode != 0)), "the float64 reference mode covers fast mode-0 descriptors"
     K = 64 * sum(d.segs[i].cblocks for i in range(d.nseg))
     rows = d.phases * d.Cout
     wts = _pair(d.weights, rows * K if split else 0, (rows, K), (K, 1))
-    if not split:
+    if not split and not f64:
         wts = wts.astype(np.float32)
     scale = np.float32(d.acc_scale if d.acc_scale != 0 else 1.0)
     bias = _view(d.bias, (d.Cout,), (1,), np.float32) if d.bias else None
     Nt, Ht, Wt = d.Nt, d.Ht, d.Wt
     hh0 = np.arange(Ht)[:, None]
     ww0 = np.arange(Wt)[None, :]
-    acc_t = np.float64 if split else np.float32
+    acc_t = np.float64 if (split or f64) else np.float32
     for phase in range(d.phases):
         pa, pb = phase >> 1, phase & 1
         acc = np.zeros((Nt, Ht, Wt, d.Cout), dtype=acc_t)
+        mag = np.zeros_like(acc) if f64 else None
         k0 = 0
         for si in range(d.nseg):
             seg = d.segs[si]
@@ -95,7 +101,24 @@ def run_desc(d):
             a[:nn, :, :, :g.shape[-1]] = g[:nn]
             wseg = wts[phase * d.Cout:(phase + 1) * d.Cout, k0:k0 + width]
             acc += np.tensordot(a, wseg, axes=([3], [1]))
+            if f64:
+                mag += np.tensordot(np.abs(a), np.abs(wseg), axes=([3], [1]))
             k0 += width
+        if f64:
+            base = d.out + 2 * (pa * d.out_pitch_h + pb * d.out_pitch_w)
+            shape = (Nt, Ht, Wt, d.Cout)
+            strides = (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1)
+            acc *= float(scale)
+            mag *= float(scale)
+            if bias is not None:
+                acc += bias
+                mag += np.abs(bias)
+            if d.residual:
+                r = _view(d.residual + 2 * (pa * d.out_pitch_h + pb * d.out_pitch_w), shape, strides).astype(np.float64)
+                acc += r
+                mag += np.abs(r)
+            sink(base, shape, strides, np.maximum(acc, 0) if d.relu else acc, mag)
+            continue
         acc = acc.astype(np.float32) * scale
         if bias is not None:
             acc += bias
@@ -197,8 +220,8 @@ def run_engine(engine, x):
 # --------------------------------------------------------------------------------------------------
 # training plan emulation (robosat_b200/train_engine.py op lists on CPU buffers)
 # --------------------------------------------------------------------------------------------------
-def _gather_segment(d, seg, phase):
-    """A operand of one segment for all tile-space pixels: float32 [Nt, Ht, Wt, 64*cblocks] (zero outside the view)"""
+def _gather_segment(d, seg, phase, dtype=np.float32):
+    """A operand of one segment for all tile-space pixels: [Nt, Ht, Wt, 64*cblocks] of `dtype` (zero outside the view)"""
     pa, pb = phase >> 1, phase & 1
     src = d.srcs[seg.src]
     width = seg.cblocks * 64
@@ -206,27 +229,37 @@ def _gather_segment(d, seg, phase):
     hh = np.arange(d.Ht)[:, None] + seg.dh + pa
     ww = np.arange(d.Wt)[None, :] + seg.dw + pb
     inb = (hh >= 0) & (hh < src.H) & (ww >= 0) & (ww < src.W)
-    g = sv[:, np.clip(hh, 0, src.H - 1), np.clip(ww, 0, src.W - 1), :].astype(np.float32) * inb[None, :, :, None]
-    a = np.zeros((d.Nt, d.Ht, d.Wt, width), dtype=np.float32)
+    g = sv[:, np.clip(hh, 0, src.H - 1), np.clip(ww, 0, src.W - 1), :].astype(dtype) * inb[None, :, :, None]
+    a = np.zeros((d.Nt, d.Ht, d.Wt, width), dtype=dtype)
     nn = min(d.Nt, src.N)
     a[:nn, :, :, :g.shape[-1]] = g[:nn]
     return a
 
 
-def run_wgrad(d, dy_ptr, dw):
-    """dw[phase*Cout + co][k] = sum_pixels dy_phase[p][co] * A_segment(k)[p]  (what rsb_wgrad_run accumulates); dw: torch fp32"""
+def run_wgrad(d, dy_ptr, dw, f64=False):
+    """dw[phase*Cout + co][k] = sum_pixels dy_phase[p][co] * A_segment(k)[p]  (what rsb_wgrad_run accumulates); dw: torch fp32.
+    f64=True: nothing is written; returns float64 (gradient, same contraction over |dy|*|A|), both [phases*Cout, K]."""
     K = 64 * sum(d.segs[i].cblocks for i in range(d.nseg))
-    out = dw.numpy().reshape(d.phases * d.Cout, K)
-    out[...] = 0
+    dt = np.float64 if f64 else np.float32
+    if f64:
+        out, mag = np.zeros((d.phases * d.Cout, K)), np.zeros((d.phases * d.Cout, K))
+    else:
+        out = dw.numpy().reshape(d.phases * d.Cout, K)
+        out[...] = 0
     for phase in range(d.phases):
         pa, pb = phase >> 1, phase & 1
         base = dy_ptr + 2 * (pa * d.out_pitch_h + pb * d.out_pitch_w)
-        dyv = _view(base, (d.Nt, d.Ht, d.Wt, d.Cout), (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1)).astype(np.float32)
+        dyv = _view(base, (d.Nt, d.Ht, d.Wt, d.Cout), (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1)).astype(dt)
         k0 = 0
         for si in range(d.nseg):
-            a = _gather_segment(d, d.segs[si], phase)
-            out[phase * d.Cout:(phase + 1) * d.Cout, k0:k0 + a.shape[-1]] = np.tensordot(dyv, a, axes=([0, 1, 2], [0, 1, 2]))
+            a = _gather_segment(d, d.segs[si], phase, dt)
+            rows = slice(phase * d.Cout, (phase + 1) * d.Cout)
+            out[rows, k0:k0 + a.shape[-1]] = np.tensordot(dyv, a, axes=([0, 1, 2], [0, 1, 2]))
+            if f64:
+                mag[rows, k0:k0 + a.shape[-1]] = np.tensordot(np.abs(dyv), np.abs(a), axes=([0, 1, 2], [0, 1, 2]))
             k0 += a.shape[-1]
+    if f64:
+        return out, mag
 
 
 def run_train_ops(eng, ops, x=None, dlogits=None):
@@ -270,6 +303,7 @@ def run_train_ops(eng, ops, x=None, dlogits=None):
             P[pf + ".running_mean"].mul_(0.9).add_(0.1 * mean.float())
             P[pf + ".running_var"].mul_(0.9).add_(0.1 * (var * b.M / (b.M - 1)).float())
             P[pf + ".num_batches_tracked"].add_(1)
+            b.sums.zero_()  # the chained kernels leave their accumulators cleared for the next call
         elif k == "bn_apply":
             _, b, res, y, relu = op
             o = b.z.reshape(b.M, b.C).float() * b.scale + b.shift
