@@ -258,6 +258,25 @@ int rsb_head_tta_argmax(const int64_t* acc, uint8_t* mask, int32_t B, int32_t C,
 /* rsb_augment_dihedral's image transform for H x W tiles without a mask; when H != W only the flip bit of each op is used */
 int rsb_augment_flip_rect(const uint8_t* img, const int32_t* ops, uint8_t* out_img, int32_t N, int32_t H, int32_t W, void* stream);
 
+/* `rs features` mask morphology (robosat/features/core.py:65-92: denoise = MORPH_OPEN, grow = MORPH_CLOSE, OpenCV semantics).
+ * A chain of up to RSB_MORPH_MAX_OPS binary erosions / dilations of m = (labels == class_index), fused: each label byte is read
+ * once and each output byte written once. Op k: out(y, x) = min (erode) or max (dilate) over the element's set cells (i, j) of
+ * in(y + i - ay, x + j - ax), no reflection; pixels outside the image are ignored (1 for erode, 0 for dilate). Row i of the
+ * element is the run of columns [span[i][0], span[i][1]), empty if span[i][0] >= span[i][1] (every row of an OpenCV ellipse,
+ * rectangle or cross is one run). ops_host is read on the host and passed by value into the launch.
+ * labels uint8 [N] images of H x W, image n at labels + n * image_stride -> out uint8 {0, 1} [N][H][W]; fg_counts int32 [N] = number
+ * of 1 pixels of each result. 1 <= H, W <= 1024, 1 <= kh, kw <= 64; allocates nothing and does not synchronise. */
+#define RSB_MORPH_MAX_OPS 4
+#define RSB_MORPH_MAX_K 64
+typedef struct rsb_morph_op {
+    int32_t dilate;                       /* 0 = erode, 1 = dilate */
+    int32_t kh, kw;                       /* element size */
+    int32_t ay, ax;                       /* anchor (OpenCV's default is (kh / 2, kw / 2)) */
+    int16_t span[RSB_MORPH_MAX_K][2];     /* rows 0 .. kh-1 are used */
+} rsb_morph_op;
+int rsb_morph_binary(const uint8_t* labels, int64_t image_stride, int32_t N, int32_t H, int32_t W, int32_t class_index,
+                     const rsb_morph_op* ops_host, int32_t nops, uint8_t* out, int32_t* fg_counts, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Host-side PNG codec for the files either side of the predict path (HOST pointers, plain C over zlib, no Python / GIL so the
  * tools' pool threads run truly in parallel). Pixel-identical to PIL; not a compute fallback -- no device work happens here.

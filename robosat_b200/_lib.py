@@ -80,6 +80,21 @@ class ConvDesc(ctypes.Structure):
     ]
 
 
+RSB_MORPH_MAX_OPS = 4
+RSB_MORPH_MAX_K = 64
+
+
+class MorphOp(ctypes.Structure):
+    _fields_ = [
+        ("dilate", ctypes.c_int32),
+        ("kh", ctypes.c_int32),
+        ("kw", ctypes.c_int32),
+        ("ay", ctypes.c_int32),
+        ("ax", ctypes.c_int32),
+        ("span", (ctypes.c_int16 * 2) * RSB_MORPH_MAX_K),
+    ]
+
+
 class RowConvDesc(ctypes.Structure):
     _fields_ = [
         ("src", ConvSrc),
@@ -144,6 +159,7 @@ SIGNATURES = {
     "rsb_head_tta_quantize": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_head_tta_argmax": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_augment_flip_rect": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "rsb_morph_binary": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, ctypes.POINTER(MorphOp), _i32, _vp, _vp, _vp]),
     "rsb_zlib_inflate": (ctypes.c_int, [ctypes.c_char_p, _i64, _vp, _i64]),
     "rsb_png_decode_rgb": (ctypes.c_int, [_vp, _i64, _vp, _i32, _i32]),
     "rsb_png_read_rgb": (ctypes.c_int, [ctypes.c_char_p, _vp, _i32, _i32]),

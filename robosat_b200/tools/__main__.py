@@ -1,9 +1,9 @@
-"""`python -m robosat_b200.tools {train,predict,serve,masks,weights} ...` -- the `rs` sub-commands on the hot path
+"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features} ...` -- the `rs` sub-commands on the hot path
 (dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
 
 import argparse
 
-from robosat_b200.tools import masks, predict, serve, train, weights
+from robosat_b200.tools import features, masks, predict, serve, train, weights
 
 
 def add_parsers():
@@ -14,6 +14,7 @@ def add_parsers():
     serve.add_parser(subparser)
     masks.add_parser(subparser)
     weights.add_parser(subparser)
+    features.add_parser(subparser)
     subparser.required = True
     return parser.parse_args()
 
