@@ -277,6 +277,23 @@ typedef struct rsb_morph_op {
 int rsb_morph_binary(const uint8_t* labels, int64_t image_stride, int32_t N, int32_t H, int32_t W, int32_t class_index,
                      const rsb_morph_op* ops_host, int32_t nops, uint8_t* out, int32_t* fg_counts, void* stream);
 
+/* `rs rasterize` polygon fill (robosat/tools/rasterize.py:64-83: rasterio.features.rasterize, all_touched=False, burn value 1,
+ * merge "replace"). All arrays are DEVICE pointers. Polygons: vertices float64 [num_vertices][2] (EPSG:3857 X, Y; 16-byte aligned);
+ * ring r owns vertices [ring_offsets[r], ring_offsets[r + 1]) and is closed implicitly; polygon p owns rings
+ * [poly_rings[p], poly_rings[p + 1]) (outer ring and holes, filled even-odd). Tile n burns polygons
+ * tile_polys[tile_poly_offsets[n] .. tile_poly_offsets[n + 1]) (ids outside [0, num_polys) are skipped) with the transform
+ * tile_transforms[n] = (c0, c1, r0, r1): px = c0 + X * c1, py = r0 + Y * r1, every float64 operation rounded separately (no FMA).
+ * Row r is filled on the line r + 0.5: an edge with y1 <= y2 crosses it iff y1 <= r + 0.5 < y2, at
+ * x = (r + 0.5 - y1) * (x2 - x1) / (y2 - y1) + x1; sorted crossings pair into column spans [floor(a + 0.5), floor(b + 0.5)) clipped
+ * to [0, size). The polygons of a tile are unioned. out uint8 {0, 1}: row y of tile n at out + n * image_stride + y * size;
+ * fg_counts int32 [N] = number of 1 pixels per tile. 1 <= size <= RSB_RASTER_MAX_SIZE; tile_polys is never NULL (pass a one-element
+ * array when no tile has a polygon), the polygon arrays may be NULL when num_polys = 0. Arguments are validated on the host before
+ * any device call; allocates nothing and does not synchronise. */
+#define RSB_RASTER_MAX_SIZE 4096
+int rsb_rasterize_polygons(const double* vertices, const int64_t* ring_offsets, const int32_t* poly_rings, int32_t num_polys,
+                           const int32_t* tile_poly_offsets, const int32_t* tile_polys, const double* tile_transforms, int32_t N, int32_t size,
+                           uint8_t* out, int64_t image_stride, int32_t* fg_counts, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Host-side PNG codec for the files either side of the predict path (HOST pointers, plain C over zlib, no Python / GIL so the
  * tools' pool threads run truly in parallel). Pixel-identical to PIL; not a compute fallback -- no device work happens here.

@@ -82,6 +82,7 @@ class ConvDesc(ctypes.Structure):
 
 RSB_MORPH_MAX_OPS = 4
 RSB_MORPH_MAX_K = 64
+RSB_RASTER_MAX_SIZE = 4096
 
 
 class MorphOp(ctypes.Structure):
@@ -160,6 +161,7 @@ SIGNATURES = {
     "rsb_head_tta_argmax": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_augment_flip_rect": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_morph_binary": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, ctypes.POINTER(MorphOp), _i32, _vp, _vp, _vp]),
+    "rsb_rasterize_polygons": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]),
     "rsb_zlib_inflate": (ctypes.c_int, [ctypes.c_char_p, _i64, _vp, _i64]),
     "rsb_png_decode_rgb": (ctypes.c_int, [_vp, _i64, _vp, _i32, _i32]),
     "rsb_png_read_rgb": (ctypes.c_int, [ctypes.c_char_p, _vp, _i32, _i32]),

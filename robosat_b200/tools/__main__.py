@@ -1,9 +1,9 @@
-"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features} ...` -- the `rs` sub-commands on the hot path
-(dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
+"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize} ...` -- the `rs` sub-commands on the hot
+path (dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
 
 import argparse
 
-from robosat_b200.tools import features, masks, predict, serve, train, weights
+from robosat_b200.tools import features, masks, predict, rasterize, serve, train, weights
 
 
 def add_parsers():
@@ -15,6 +15,7 @@ def add_parsers():
     masks.add_parser(subparser)
     weights.add_parser(subparser)
     features.add_parser(subparser)
+    rasterize.add_parser(subparser)
     subparser.required = True
     return parser.parse_args()
 
