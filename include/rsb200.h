@@ -323,6 +323,43 @@ int rsb_cover_emit_keys(const uint32_t* bitmap, int64_t bitmap_words, const int6
 int64_t rsb_sort_unique_workspace_bytes(int64_t n);
 int rsb_sort_unique_u64(int64_t* keys, int64_t n, int32_t key_bits, void* workspace, int64_t workspace_bytes, int64_t* unique_count, void* stream);
 
+/* `rs dedupe` (robosat/tools/dedupe.py, robosat/spatial/core.py; the rule is DESIGN.md §8). A set of features as DEVICE arrays
+ * (the struct itself is a HOST pointer): vertices double [num_vertices][2], 16-byte aligned; next int32 [num_vertices], the
+ * vertex the edge from v ends at (rings close implicitly and repeat no vertex consecutively; exterior rings counter-clockwise
+ * and holes clockwise in projected coordinates); feature f's edges start at vertices [feature_vertices[f], feature_vertices[f + 1]);
+ * exteriors[exterior_offsets[f] .. exterior_offsets[f + 1]) are the first vertices of its components' exterior rings; boxes
+ * double [num_features][4] = (xmin, ymin, xmax, ymax) of its vertices. A y-band index of the edges (read by rsb_dedupe_areas):
+ * feature f has nb = feature_bands[f + 1] - feature_bands[f] bands (0: no index, its edges are scanned in full); y maps to band
+ * clamp(floor((y - band_ranges[f][0]) * band_ranges[f][1]), 0, nb - 1), and band b lists in band_edges[band_offsets[fb + b] ..
+ * band_offsets[fb + b + 1]) (fb = feature_bands[f]) the first vertices of the edges whose y ranges meet it. */
+typedef struct RsbShapes {
+    const double* vertices;
+    const int32_t* next;
+    const int64_t* feature_vertices;
+    const int64_t* exterior_offsets;
+    const int64_t* exteriors;
+    const double* boxes;
+    const int64_t* feature_bands;
+    const double* band_ranges;
+    const int64_t* band_offsets;
+    const int32_t* band_edges;
+    int64_t num_vertices;
+    int32_t num_features;
+    int32_t reserved;
+} RsbShapes;
+/* out[i] = 1 when predicted feature pairs[i][0] and OSM feature pairs[i][1] are not disjoint (GEOS `intersects`: some edges
+ * meet, touching included, or one lies inside the other), else 0; exact orientation predicates on the lon/lat vertices. */
+int rsb_dedupe_intersects(const RsbShapes* predicted, const RsbShapes* osm, const int32_t* pairs, int64_t num_pairs, uint8_t* out, void* stream);
+/* For B predictions b (feature pred[b]) with the OSM features S(b) = set_ids[set_offsets[b] .. set_offsets[b + 1]) (ascending,
+ * set_offsets[0] = 0): areas double [B][3] = (A(P), A(P ∩ U), A(U)) of P and U = the union of S(b), on projected vertices relative
+ * to origins double [B][2]. The work items are the edges of P then those of each feature of S(b): segment b + set_offsets[b] is
+ * P's, segment b + set_offsets[b] + 1 + k is S(b)[k]'s; item_offsets int64 [num_segments + 1] (item_offsets[0] = 0) gives each
+ * segment's items (one per edge of its feature) and segment_pred int32 [num_segments] its b. terms: DEVICE double
+ * [2 * num_items] workspace. Sums run in item order, so the result is identical from run to run and across batches. */
+int rsb_dedupe_areas(const RsbShapes* predicted, const RsbShapes* osm, int32_t B, const int32_t* pred, const double* origins, const int64_t* set_offsets,
+                     const int32_t* set_ids, int64_t num_segments, const int64_t* item_offsets, const int32_t* segment_pred, int64_t num_items,
+                     double* terms, double* areas, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Host-side PNG codec for the files either side of the predict path (HOST pointers, plain C over zlib, no Python / GIL so the
  * tools' pool threads run truly in parallel). Pixel-identical to PIL; not a compute fallback -- no device work happens here.

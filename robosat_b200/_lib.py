@@ -132,6 +132,26 @@ class RowConvDesc(ctypes.Structure):
     ]
 
 
+class Shapes(ctypes.Structure):
+    """RsbShapes: a packed feature set for rsb_dedupe_intersects / rsb_dedupe_areas (device pointers)"""
+
+    _fields_ = [
+        ("vertices", ctypes.c_void_p),
+        ("next", ctypes.c_void_p),
+        ("feature_vertices", ctypes.c_void_p),
+        ("exterior_offsets", ctypes.c_void_p),
+        ("exteriors", ctypes.c_void_p),
+        ("boxes", ctypes.c_void_p),
+        ("feature_bands", ctypes.c_void_p),
+        ("band_ranges", ctypes.c_void_p),
+        ("band_offsets", ctypes.c_void_p),
+        ("band_edges", ctypes.c_void_p),
+        ("num_vertices", ctypes.c_int64),
+        ("num_features", ctypes.c_int32),
+        ("reserved", ctypes.c_int32),
+    ]
+
+
 # name -> (restype, argtypes); mirrors include/rsb200.h one to one (tests/test_abi.py checks both sides)
 _vp, _i32, _i64, _f32 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float
 SIGNATURES = {
@@ -168,6 +188,8 @@ SIGNATURES = {
     "rsb_cover_emit_keys": (ctypes.c_int, [_vp, _i64, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]),
     "rsb_sort_unique_workspace_bytes": (_i64, [_i64]),
     "rsb_sort_unique_u64": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i64, _vp, _vp]),
+    "rsb_dedupe_intersects": (ctypes.c_int, [ctypes.POINTER(Shapes), ctypes.POINTER(Shapes), _vp, _i64, _vp, _vp]),
+    "rsb_dedupe_areas": (ctypes.c_int, [ctypes.POINTER(Shapes), ctypes.POINTER(Shapes), _i32, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp]),
     "rsb_zlib_inflate":(ctypes.c_int, [ctypes.c_char_p, _i64, _vp, _i64]),
     "rsb_png_decode_rgb": (ctypes.c_int, [_vp, _i64, _vp, _i32, _i32]),
     "rsb_png_read_rgb": (ctypes.c_int, [ctypes.c_char_p, _vp, _i32, _i32]),

@@ -68,6 +68,21 @@ class PolygonSet:
         np.cumsum([len(r) for r in rings], out=self.ring_offsets[1:])
         self.poly_rings = np.zeros(len(polygons) + 1, np.int32)
         np.cumsum([len(p) for p in polygons], out=self.poly_rings[1:])
+        self._finish(device)
+
+    @classmethod
+    def from_arrays(cls, vertices, ring_offsets, poly_rings, device=None):
+        """A PolygonSet of already packed arrays: float64 vertices [V, 2], int64 ring offsets [R + 1], int32 polygon -> ring
+        offsets [P + 1]."""
+        self = cls.__new__(cls)
+        self.vertices = np.ascontiguousarray(vertices, dtype=np.float64).reshape(-1, 2)
+        self.ring_offsets = np.ascontiguousarray(ring_offsets, dtype=np.int64)
+        self.poly_rings = np.ascontiguousarray(poly_rings, dtype=np.int32)
+        self._finish(device)
+        return self
+
+    def _finish(self, device):
+        polygons = range(len(self.poly_rings) - 1)
         self.bboxes = np.full((len(polygons), 4), np.nan)
         starts, ends = self.ring_offsets[self.poly_rings[:-1]], self.ring_offsets[self.poly_rings[1:]]
         full = np.flatnonzero(ends > starts)
