@@ -360,6 +360,32 @@ int rsb_dedupe_areas(const RsbShapes* predicted, const RsbShapes* osm, int32_t B
                      const int32_t* set_ids, int64_t num_segments, const int64_t* item_offsets, const int32_t* segment_pred, int64_t num_items,
                      double* terms, double* areas, void* stream);
 
+/* `rs merge` (robosat/tools/merge.py, robosat/graph/core.py; the rule is DESIGN.md §8). All arrays are DEVICE pointers.
+ * rsb_merge_near: out[i] = 1 when features pairs[i][0] and pairs[i][1] of `shapes` (RsbShapes on EPSG:3395 vertices; the band
+ * index is not read) are within `threshold` of each other: some vertex of one has |p - q|^2 <= threshold^2 to the nearest point q
+ * of some edge of the other, q = a + clamp(((p - a).(b - a)) / |b - a|^2, 0, 1) (b - a), every float64 operation rounded on its
+ * own. */
+int rsb_merge_near(const RsbShapes* shapes, const int32_t* pairs, int64_t num_pairs, double threshold, uint8_t* out, void* stream);
+/* Connected components of n nodes under the pairs i with linked[i] != 0: labels int32 [n] = the smallest node of each node's
+ * component, the same on every run. parent: int32 [n] workspace. */
+int rsb_merge_components(const int32_t* pairs, const uint8_t* linked, int64_t num_pairs, int32_t n, int32_t* parent, int32_t* labels, void* stream);
+/* Cell fill of C components on their own grids: component c fills polygons comp_polys[comp_poly_offsets[c] .. comp_poly_offsets[c + 1])
+ * of the polygon arrays of rsb_rasterize_polygons (even-odd per polygon, union across polygons) with rsb_rasterize_polygons's
+ * scanline rule under transforms[c] = (c0, c1, r0, r1) (px = c0 + X * c1, py = r0 + Y * r1, no FMA). grids int64 [C][2] = (W, H);
+ * rows of ceil(W / 32) uint32 words at bitmap + bitmap_offsets[c], bit b of word w = column 32 w + b. One CTA per band: bands
+ * int32 [num_bands][3] = (component, first row, rows <= band_rows), covering every row once; max_words >= every ceil(W / 32),
+ * band_rows * max_words <= RSB_COVER_MAX_WIDTH / 32. The bitmap (bitmap_words words) is cleared here. */
+int rsb_merge_fill(const double* vertices, const int64_t* ring_offsets, const int32_t* poly_rings, int32_t num_polys,
+                   const int32_t* comp_poly_offsets, const int32_t* comp_polys, const double* transforms, const int64_t* grids,
+                   const int64_t* bitmap_offsets, int32_t C, const int32_t* bands, int32_t num_bands, int32_t band_rows, int32_t max_words,
+                   uint32_t* bitmap, int64_t bitmap_words, void* stream);
+/* Closing erode(dilate(fill)) with the disk {(i, j): i^2 + j^2 <= radius^2}, cells outside a grid counting as 0, into out (same
+ * layout as fill, not aliasing it); counts int64 [C] = set cells of each closed grid. One CTA per tile: tiles int32
+ * [num_tiles][3] = (component, first row, first word) of 32 rows x 32 words, covering every grid. 1 <= radius <= RSB_MERGE_MAX_RADIUS. */
+#define RSB_MERGE_MAX_RADIUS 16
+int rsb_merge_close(const uint32_t* fill, const int64_t* grids, const int64_t* bitmap_offsets, int32_t C, const int32_t* tiles, int32_t num_tiles,
+                    int32_t radius, uint32_t* out, int64_t* counts, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Host-side PNG codec for the files either side of the predict path (HOST pointers, plain C over zlib, no Python / GIL so the
  * tools' pool threads run truly in parallel). Pixel-identical to PIL; not a compute fallback -- no device work happens here.

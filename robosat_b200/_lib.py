@@ -85,6 +85,7 @@ RSB_MORPH_MAX_K = 64
 RSB_RASTER_MAX_SIZE = 4096
 RSB_COVER_MAX_WIDTH = 1856000
 RSB_COVER_MAX_ZOOM = 30
+RSB_MERGE_MAX_RADIUS = 16
 
 
 class MorphOp(ctypes.Structure):
@@ -190,6 +191,10 @@ SIGNATURES = {
     "rsb_sort_unique_u64": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i64, _vp, _vp]),
     "rsb_dedupe_intersects": (ctypes.c_int, [ctypes.POINTER(Shapes), ctypes.POINTER(Shapes), _vp, _i64, _vp, _vp]),
     "rsb_dedupe_areas": (ctypes.c_int, [ctypes.POINTER(Shapes), ctypes.POINTER(Shapes), _i32, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp]),
+    "rsb_merge_near": (ctypes.c_int, [ctypes.POINTER(Shapes), _vp, _i64, ctypes.c_double, _vp, _vp]),
+    "rsb_merge_components": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "rsb_merge_fill": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _i64, _vp]),
+    "rsb_merge_close": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
     "rsb_zlib_inflate":(ctypes.c_int, [ctypes.c_char_p, _i64, _vp, _i64]),
     "rsb_png_decode_rgb": (ctypes.c_int, [_vp, _i64, _vp, _i32, _i32]),
     "rsb_png_read_rgb": (ctypes.c_int, [ctypes.c_char_p, _vp, _i32, _i32]),

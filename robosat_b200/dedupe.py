@@ -78,9 +78,10 @@ class ShapeSet:
     [feature_polys[f], feature_polys[f + 1]) of `lonlat` and `xy` (rasterize.PolygonSets with the same offsets). Rings hold no
     two equal consecutive projected vertices and no closing repeat; `next[v]` is the vertex the edge from v ends at. Exterior
     rings run counter-clockwise and holes clockwise in (x, y). `feature_vertices`, `exterior_offsets` / `exteriors` and the
-    per-feature boxes (`boxes_ll`, `boxes_xy`, NaN for a feature without vertices) are what the kernels read."""
+    per-feature boxes (`boxes_ll`, `boxes_xy`, NaN for a feature without vertices) are what the kernels read. `projection` maps
+    lon/lat to the (x, y) of `xy`: Mollweide for dedupe, EPSG:3395 for `rs merge`."""
 
-    def __init__(self, polygons_per_feature, index):
+    def __init__(self, polygons_per_feature, index, projection=mollweide):
         self.index = np.asarray(index, np.int64)
         counts = [len(p) for p in polygons_per_feature]
         self.feature_polys = np.zeros(len(counts) + 1, np.int64)
@@ -88,7 +89,7 @@ class ShapeSet:
         raw = PolygonSet([p for ps in polygons_per_feature for p in ps])
         ro, V = raw.ring_offsets, raw.vertices
         nr = len(ro) - 1
-        xy = mollweide(V)
+        xy = projection(V)
         rid = np.repeat(np.arange(nr), np.diff(ro))
         idx = np.arange(len(V))
         succ = np.where(idx + 1 < ro[rid + 1], idx + 1, ro[rid])

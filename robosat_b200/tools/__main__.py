@@ -1,9 +1,9 @@
-"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe} ...` -- the `rs` sub-commands on the
+"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe,merge} ...` -- the `rs` sub-commands on the
 hot path (dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
 
 import argparse
 
-from robosat_b200.tools import cover, dedupe, features, masks, predict, rasterize, serve, train, weights
+from robosat_b200.tools import cover, dedupe, features, masks, merge, predict, rasterize, serve, train, weights
 
 
 def add_parsers():
@@ -18,6 +18,7 @@ def add_parsers():
     rasterize.add_parser(subparser)
     cover.add_parser(subparser)
     dedupe.add_parser(subparser)
+    merge.add_parser(subparser)
     subparser.required = True
     return parser.parse_args()
 
