@@ -387,6 +387,105 @@ int rsb_merge_close(const uint32_t* fill, const int64_t* grids, const int64_t* b
                     int32_t radius, uint32_t* out, int64_t* counts, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * `rs extract` (robosat/tools/extract.py, robosat/osm/{core,parking,building}.py; the rule is DESIGN.md §8): OpenStreetMap PBF files.
+ * Host entry points (HOST pointers, plain C++ over zlib, csrc/rsb_pbf.cpp) frame, inflate and parse; the device entry points
+ * (csrc/rsb_extract.cu) decode DenseNodes, join node locations to way refs and check ring validity.
+ *
+ * rsb_pbf_frames: lists the [uint32 BE length][BlobHeader][Blob] frames of file_host[0 .. n) into frames_host int64
+ * [capacity][RSB_PBF_FRAME_FIELDS] = (kind, compression, data offset, data length, raw_size, frame offset); *count_host = the number of
+ * frames (only the first `capacity` are written). Errors: a truncated frame, a BlobHeader of 64 KiB or more, a Blob or raw_size over
+ * 32 MiB, malformed messages.
+ * rsb_pbf_inflate: blob i (frames_host row i) -> out_host + out_offsets_host[i], exactly raw_size bytes, with RSB_PBF_INFLATE_PAD
+ * writable bytes after each; `threads` threads. raw and zlib_data are supported; any other compression, a corrupt zlib stream or an
+ * inflated size other than raw_size is an error naming the blob.
+ * rsb_pbf_check_header: an OSMHeader's HeaderBlock; a required feature other than OsmSchema-V0.6 and DenseNodes is an error naming it.
+ * rsb_pbf_parse: the PrimitiveBlocks blocks_host + offsets_host[i] (sizes_host[i] bytes) -> *result (free with rsb_pbf_result_free;
+ * read with rsb_pbf_result_sizes / rsb_pbf_result_copy, element counts of RSB_PBF_OUT_*):
+ *   RSB_PBF_WAYS: keys_host = nkeys NUL-terminated keys back to back; keys[0] is the anchor. The ways whose first keys[0] tag exists
+ *     (and equals anchor_value_host, unless that is NULL or empty), in file order: WAY_IDS int64 [W], REF_OFFSETS int64 [W + 1],
+ *     REFS int64 node ids (delta-decoded), TAGS int32 [W][nkeys] = index of the key's first value in STRING_OFFSETS int64 [S + 1] /
+ *     STRING_BYTES, or -1. KINDS int32 [n] = RSB_PBF_HAS_* bits of each block.
+ *   RSB_PBF_NODES: SEGS int64 [G][RSB_PBF_SEG_FIELDS], the node runs of the blocks in element order: kind 0 is a DenseNodes group
+ *     whose packed id / lat / lon fields lie at the given offsets from its block's start (COUNT values each), kind 1 a run of COUNT
+ *     nodes decoded here into HOST_IDS int64 / HOST_XY int32 [][2] from HOST_FIRST (plain Nodes, and DenseNodes with unpacked fields).
+ *     Coordinates: x = (lon * granularity + lon_offset) / 100 in int64 (truncating), INT32_MIN outside +-180e7; y likewise with
+ *     lat, +-90e7. */
+#define RSB_PBF_FRAME_FIELDS 6
+#define RSB_PBF_BLOB_HEADER 0
+#define RSB_PBF_BLOB_DATA 1
+#define RSB_PBF_BLOB_OTHER 2
+#define RSB_PBF_RAW 0
+#define RSB_PBF_ZLIB 1
+#define RSB_PBF_NO_DATA 6
+#define RSB_PBF_INFLATE_PAD 64
+#define RSB_PBF_WAYS 0
+#define RSB_PBF_NODES 1
+#define RSB_PBF_MAX_KEYS 8
+#define RSB_PBF_HAS_NODES 1
+#define RSB_PBF_HAS_DENSE 2
+#define RSB_PBF_HAS_WAYS 4
+#define RSB_PBF_HAS_RELATIONS 8
+#define RSB_PBF_OUT_KINDS 0
+#define RSB_PBF_OUT_WAY_IDS 1
+#define RSB_PBF_OUT_REF_OFFSETS 2
+#define RSB_PBF_OUT_REFS 3
+#define RSB_PBF_OUT_TAGS 4
+#define RSB_PBF_OUT_STRING_OFFSETS 5
+#define RSB_PBF_OUT_STRING_BYTES 6
+#define RSB_PBF_OUT_SEGS 7
+#define RSB_PBF_OUT_HOST_IDS 8
+#define RSB_PBF_OUT_HOST_XY 9
+#define RSB_PBF_OUT_COUNT 10
+#define RSB_PBF_SEG_FIELDS 16
+#define RSB_PBF_SEG_BLOCK 0
+#define RSB_PBF_SEG_KIND 1
+#define RSB_PBF_SEG_COUNT 2
+#define RSB_PBF_SEG_ID_OFF 3
+#define RSB_PBF_SEG_ID_LEN 4
+#define RSB_PBF_SEG_LAT_OFF 5
+#define RSB_PBF_SEG_LAT_LEN 6
+#define RSB_PBF_SEG_LON_OFF 7
+#define RSB_PBF_SEG_LON_LEN 8
+#define RSB_PBF_SEG_GRANULARITY 9
+#define RSB_PBF_SEG_LAT_OFFSET 10
+#define RSB_PBF_SEG_LON_OFFSET 11
+#define RSB_PBF_SEG_HOST_FIRST 12
+#define RSB_PBF_SEG_OUT_FIRST 13
+int rsb_pbf_frames(const uint8_t* file_host, int64_t n, int64_t* frames_host, int64_t capacity, int64_t* count_host);
+int rsb_pbf_inflate(const uint8_t* file_host, const int64_t* frames_host, int32_t n, uint8_t* out_host, const int64_t* out_offsets_host, int32_t threads);
+int rsb_pbf_check_header(const uint8_t* block_host, int64_t n);
+int rsb_pbf_parse(const uint8_t* blocks_host, const int64_t* offsets_host, const int64_t* sizes_host, int32_t n, int32_t mode, const char* keys_host,
+                  int32_t nkeys, const char* anchor_value_host, int32_t threads, void** result);
+int rsb_pbf_result_sizes(const void* result, int64_t* sizes_host);
+int rsb_pbf_result_copy(const void* result, int32_t what, void* dst_host, int64_t count);
+void rsb_pbf_result_free(void* result);
+/* Device. rsb_pbf_dense_nodes: decodes the DenseNodes segments (kind 0 rows of rsb_pbf_parse's SEGS, DEVICE int64 [G][RSB_PBF_SEG_FIELDS],
+ * offsets relative to blocks + block_offsets[SEG_BLOCK], blocks padded by RSB_PBF_INFLATE_PAD readable bytes) into records
+ * SEG_OUT_FIRST .. + COUNT of ids int64 [] and xy int32 [][2] (coordinates as above). Varints of up to 10 bytes; status int32 [1] is
+ * cleared and then set non-zero for a varint longer than 10 bytes or a segment that does not hold COUNT values. */
+int rsb_pbf_dense_nodes(const uint8_t* blocks, const int64_t* block_offsets, const int64_t* segs, int32_t G, int64_t* ids, int32_t* xy, int32_t* status,
+                        void* stream);
+/* rsb_extract_locate: for node records i < n (ids int64, xy int32 [n][2]) of global ordinal ordinal_base + i, whose biased id
+ * (id XOR 2^63, as uint64) is found in the ascending unique keys[0 .. num_keys), best[k] = max(best[k], ordinal + 1) and then, where
+ * that ordinal won, loc[k] = xy[i]: the last record of an id in file order wins. best (uint64, zero = not seen) and loc (int32 [][2])
+ * persist across calls made in file order. */
+int rsb_extract_locate(const int64_t* ids, const int32_t* xy, int64_t n, int64_t ordinal_base, const int64_t* keys, int64_t num_keys, int64_t* best,
+                       int32_t* loc, void* stream);
+/* rsb_extract_gather: for refs i < num_refs (biased ids) of way ref_way[i] < num_ways: verts int32 [num_refs][2] = the location of the ref;
+ * flags int32 [num_ways] (cleared here) |= 1 for a ref not in keys or never located, 2 for an invalid location. */
+int rsb_extract_gather(const int64_t* refs, const int32_t* ref_way, int64_t num_refs, int32_t num_ways, const int64_t* keys, int64_t num_keys,
+                       const int64_t* best, const int32_t* loc, int32_t* verts, int32_t* flags, void* stream);
+/* rsb_extract_valid: `features.polygon_is_valid([ring])` for rings r < R (verts int32 [][2] from ring_offsets[r] to ring_offsets[r + 1],
+ * closed: the last vertex repeats the first) on the integer lattice, exactly: after dropping the closing vertex and consecutive
+ * repeats (the compacted ring goes to scratch int32 [][2] at the same offsets, its length to lens int32 [R]), >= 3 distinct
+ * positions, non-zero area, and no two edges meet except adjacent edges in their shared vertex. Rings with flags[r] != 0 are
+ * skipped (valid 0). Rings of more than RSB_EXTRACT_WARP_RING vertices are checked pair tile by pair tile: long int32 [L] lists
+ * them (ascending), tile_offsets int64 [L + 1] the prefix of their tile counts ceil(n / 64)^2. valid uint8 [R]. */
+#define RSB_EXTRACT_WARP_RING 256
+int rsb_extract_valid(const int32_t* verts, const int64_t* ring_offsets, int32_t R, const int32_t* flags, const int32_t* long_rings, int32_t L,
+                      const int64_t* tile_offsets, int32_t* scratch, int32_t* lens, uint8_t* valid, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Host-side PNG codec for the files either side of the predict path (HOST pointers, plain C over zlib, no Python / GIL so the
  * tools' pool threads run truly in parallel). Pixel-identical to PIL; not a compute fallback -- no device work happens here.
  */

@@ -86,6 +86,19 @@ RSB_RASTER_MAX_SIZE = 4096
 RSB_COVER_MAX_WIDTH = 1856000
 RSB_COVER_MAX_ZOOM = 30
 RSB_MERGE_MAX_RADIUS = 16
+# rs extract (include/rsb200.h)
+RSB_PBF_FRAME_FIELDS = 6
+RSB_PBF_BLOB_HEADER, RSB_PBF_BLOB_DATA, RSB_PBF_BLOB_OTHER = 0, 1, 2
+RSB_PBF_INFLATE_PAD = 64
+RSB_PBF_WAYS, RSB_PBF_NODES = 0, 1
+RSB_PBF_HAS_NODES, RSB_PBF_HAS_DENSE, RSB_PBF_HAS_WAYS, RSB_PBF_HAS_RELATIONS = 1, 2, 4, 8
+(RSB_PBF_OUT_KINDS, RSB_PBF_OUT_WAY_IDS, RSB_PBF_OUT_REF_OFFSETS, RSB_PBF_OUT_REFS, RSB_PBF_OUT_TAGS, RSB_PBF_OUT_STRING_OFFSETS,
+ RSB_PBF_OUT_STRING_BYTES, RSB_PBF_OUT_SEGS, RSB_PBF_OUT_HOST_IDS, RSB_PBF_OUT_HOST_XY, RSB_PBF_OUT_COUNT) = range(11)
+RSB_PBF_SEG_FIELDS = 16
+(RSB_PBF_SEG_BLOCK, RSB_PBF_SEG_KIND, RSB_PBF_SEG_COUNT, RSB_PBF_SEG_ID_OFF, RSB_PBF_SEG_ID_LEN, RSB_PBF_SEG_LAT_OFF, RSB_PBF_SEG_LAT_LEN,
+ RSB_PBF_SEG_LON_OFF, RSB_PBF_SEG_LON_LEN, RSB_PBF_SEG_GRANULARITY, RSB_PBF_SEG_LAT_OFFSET, RSB_PBF_SEG_LON_OFFSET, RSB_PBF_SEG_HOST_FIRST,
+ RSB_PBF_SEG_OUT_FIRST) = range(14)
+RSB_EXTRACT_WARP_RING = 256
 
 
 class MorphOp(ctypes.Structure):
@@ -195,6 +208,17 @@ SIGNATURES = {
     "rsb_merge_components": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _vp]),
     "rsb_merge_fill": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _i64, _vp]),
     "rsb_merge_close": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
+    "rsb_pbf_frames": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp]),
+    "rsb_pbf_inflate": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp, _i32]),
+    "rsb_pbf_check_header": (ctypes.c_int, [_vp, _i64]),
+    "rsb_pbf_parse": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, ctypes.c_char_p, _i32, ctypes.c_char_p, _i32, ctypes.POINTER(_vp)]),
+    "rsb_pbf_result_sizes": (ctypes.c_int, [_vp, _vp]),
+    "rsb_pbf_result_copy": (ctypes.c_int, [_vp, _i32, _vp, _i64]),
+    "rsb_pbf_result_free": (None, [_vp]),
+    "rsb_pbf_dense_nodes": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "rsb_extract_locate": (ctypes.c_int, [_vp, _vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp]),
+    "rsb_extract_gather": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "rsb_extract_valid": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "rsb_zlib_inflate":(ctypes.c_int, [ctypes.c_char_p, _i64, _vp, _i64]),
     "rsb_png_decode_rgb": (ctypes.c_int, [_vp, _i64, _vp, _i32, _i32]),
     "rsb_png_read_rgb": (ctypes.c_int, [ctypes.c_char_p, _vp, _i32, _i32]),
