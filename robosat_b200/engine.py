@@ -645,18 +645,24 @@ class UNetEngine:
         Returns the engine-owned fp32 NCHW logits buffer (valid until the next call)."""
         if self.plan_only:
             raise _lib.RsbError("UNetEngine was built with plan_only=True; there is no CPU execution path")
-        lib = _lib.load()
         N, H, W = self.N, self.H, self.W
         if x.dtype == torch.float32:
             assert tuple(x.shape) == (N, 3, H, W) and x.is_contiguous() and x.is_cuda, "expected contiguous cuda fp32 [N,3,H,W]"
-            kind = 0
         elif x.dtype == torch.uint8:
             assert tuple(x.shape) == (N, H, W, 3) and x.is_contiguous() and x.is_cuda, "expected contiguous cuda uint8 [N,H,W,3]"
-            kind = 1
         else:
             raise TypeError("unsupported input dtype %s" % x.dtype)
+        self.run_ops(self.ops, x)
+        return self.logits
+
+    def run_ops(self, ops, x):
+        """Launch `ops` (entries of self.ops, in order) on the current stream; `x` is forward's validated input, read by the
+        pre-pass. forward() is run_ops(self.ops, x); a sub-list runs single launches (tests/predict_lockstep.py)."""
+        lib = _lib.load()
+        N, H, W = self.N, self.H, self.W
+        kind = 1 if x.dtype == torch.uint8 else 0
         stream = _lib.current_stream_ptr()
-        for op in self.ops:
+        for op in ops:
             if op[0] == "conv":
                 op[1].run(stream)
             elif op[0] == "prepass":
@@ -672,7 +678,6 @@ class UNetEngine:
                                "rsb_maxpool_nhwc_split")
                 else:
                     _lib.check(lib.rsb_maxpool_nhwc(src.data_ptr(), dst.data_ptr(), n, h, w, c, k, s, p, stream), "rsb_maxpool_nhwc")
-        return self.logits
 
     def feature_nchw(self, name):
         """Debug/parity view of an intermediate as fp32 NCHW on the CPU (strict mode: hi + lo)."""

@@ -42,7 +42,12 @@ def add_parser(subparser):
 
 NATIVE_PNG = os.environ.get("RSB_PNG_ENCODER", "native") != "pil"
 PNG_LEVEL = min(9, max(0, int(os.environ.get("RSB_PNG_LEVEL", "6"))))  # zlib level of the library encoder (3: ~40 % less encode time, files 4 - 16 % larger)
-_PALETTE_BYTES = {}
+
+
+def _palette_bytes(palette):
+    """the PLTE payload of a flat palette list (<= 256 entries). Converted on every call: a cache keyed by id(palette) handed
+    a later palette the bytes of an earlier, freed list that had occupied the same address"""
+    return bytes(palette[:768])
 
 
 def _save_png(root, palette, x, y, z, quantized, stats=None):
@@ -56,9 +61,7 @@ def _save_png(root, palette, x, y, z, quantized, stats=None):
     if NATIVE_PNG:
         from robosat_b200 import _lib
 
-        pal = _PALETTE_BYTES.get(id(palette))
-        if pal is None:
-            pal = _PALETTE_BYTES.setdefault(id(palette), bytes(palette[:768]))
+        pal = _palette_bytes(palette)
         q = quantized if quantized.flags["C_CONTIGUOUS"] else quantized.copy()
         _lib.check(_lib.load().rsb_png_write_p8(os.fsencode(path), q.ctypes.data, q.shape[1], q.shape[0], pal, len(pal) // 3, PNG_LEVEL), "rsb_png_write_p8")
     else:
@@ -82,9 +85,7 @@ def _save_batch(root, palette, tiles, quantized, threads, stats=None):
 
     t0 = time.perf_counter()
     n = len(tiles)
-    pal = _PALETTE_BYTES.get(id(palette))
-    if pal is None:
-        pal = _PALETTE_BYTES.setdefault(id(palette), bytes(palette[:768]))
+    pal = _palette_bytes(palette)
     paths = (ctypes.c_char_p * n)(*[os.fsencode(os.path.join(root, str(z), str(x), str(y) + ".png")) for x, y, z in tiles])
     q = quantized if quantized.flags["C_CONTIGUOUS"] else quantized.copy()
     _lib.check(_lib.load().rsb_png_write_p8_batch(paths, n, q.ctypes.data, q.shape[1] * q.shape[2], q.shape[2], q.shape[1], pal, len(pal) // 3, PNG_LEVEL,

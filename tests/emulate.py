@@ -60,65 +60,143 @@ def _pair(ptr, plane, shape, strides):
     return v
 
 
+def _operand(ptr, plane, shape, strides):
+    """float64 (hi, lo) planes of an operand view; lo is None for a single fp16 operand (plane 0)"""
+    hi = _view(ptr, shape, strides).astype(np.float64)
+    return hi, (_view(ptr + 2 * plane, shape, strides).astype(np.float64) if plane else None)
+
+
+class _F64Acc:
+    """float64 replay of one output phase, added up term by term (a: (hi, lo) [..., k], w: (hi, lo) [Cout, k]):
+      val   the contraction of the operands' values (hi + lo in split mode);
+      dot   sum (|a_hi| + |a_lo|)(|w_hi| + |w_lo|) >= sum |a||w| (fast mode: sum |a||w|), the magnitude that scales the
+            kernel's accumulation error;
+      split mode only: lolo = sum |a_lo||w_lo| (the product the kernel omits) and hihi = sum |a_hi||w_hi| (the main chain of
+            the N-concatenated schedule; dot - hihi - lolo is its cross chain)."""
+
+    def __init__(self, split):
+        self.split = split
+        self.val = self.dot = self.lolo = self.hihi = 0.0
+
+    def add(self, a, w):
+        (ah, al), (wh, wl) = a, w
+
+        def td(x, y):
+            return np.tensordot(x, y, axes=([x.ndim - 1], [1]))
+
+        if not self.split:
+            self.val = self.val + td(ah, wh)
+            self.dot = self.dot + td(np.abs(ah), np.abs(wh))
+            return
+        aa, wa, la, lw = np.abs(ah), np.abs(wh), np.abs(al), np.abs(wl)
+        self.val = self.val + td(ah + al, wh + wl)
+        self.dot = self.dot + td(aa + la, wa + lw)
+        self.lolo = self.lolo + td(la, lw)
+        self.hihi = self.hihi + td(aa, wa)
+
+
+def _f64_emit(d, acc, scale, out, shape, strides, res, out_plane, res_plane, sink):
+    """the float64 epilogue of one output phase: * acc_scale, + bias, (mode 0) + residual, ReLU; mode 1 contracts ReLU(conv),
+    kept in float64, with `final`'s fp32 weights. sink(ptr, shape, strides, value, mag, parts, plane):
+      mode 0: value [Nt, Ht, Wt, Cout] at `out` (and its lo plane `plane` elements further in split mode), mag = dot + |bias|
+              + |residual|, parts = the magnitudes of _F64Acc times acc_scale;
+      mode 1: the logits [Nt, classes, Ht, Wt] at head_out, mag = sum_c |w_c y_c| + |b|, parts = sum_c |w_c| part_c, the
+              conv's magnitudes carried through the 1x1 head (ReLU is 1-Lipschitz), with |bias| added to dot."""
+    parts = {"dot": acc.dot * scale}
+    if acc.split:
+        parts.update(lolo=acc.lolo * scale, hihi=acc.hihi * scale)
+    v = acc.val * scale
+    mag = parts["dot"]
+    if d.bias:
+        b = _view(d.bias, (d.Cout,), (1,), np.float32).astype(np.float64)
+        v, mag = v + b, mag + np.abs(b)
+    if d.mode == 0:
+        if res:
+            r = _pair(res, res_plane, shape, strides)
+            v, mag = v + r, mag + np.abs(r)
+        sink(out, shape, strides, np.maximum(v, 0) if d.relu else v, mag, parts, out_plane)
+        return
+    parts["dot"] = mag
+    y = np.maximum(v, 0) if d.relu else v
+    hw = _view(d.head_w, (d.head_classes, 32), (32, 1), np.float32).astype(np.float64)
+    hb = _view(d.head_b, (d.head_classes,), (1,), np.float32).astype(np.float64)
+
+    def head(t, w):
+        return np.transpose(np.tensordot(t, w, axes=([3], [1])), (0, 3, 1, 2))
+
+    logits = head(y, hw) + hb[None, :, None, None]
+    lmag = head(np.abs(y), np.abs(hw)) + np.abs(hb)[None, :, None, None]
+    Nt, Ht, Wt = shape[:3]
+    sink(d.head_out, (Nt, d.head_classes, Ht, Wt), (d.head_classes * Ht * Wt, Ht * Wt, Wt, 1), logits, lmag,
+         {k: head(p, np.abs(hw)) for k, p in parts.items()}, 0)
+
+
+def _run_desc_f64(d, sink):
+    split = bool(d.split)
+    K = 64 * sum(d.segs[i].cblocks for i in range(d.nseg))
+    rows = d.phases * d.Cout
+    w = _operand(d.weights, rows * K if split else 0, (rows, K), (K, 1))
+    srcs = [_operand(s.ptr, s.plane if split else 0, (s.N, s.H, s.W, s.C), (s.pitch_n, s.pitch_h, s.pitch_w, 1))
+            for s in (d.srcs[i] for i in range(d.nsrc))]
+    for phase in range(d.phases):
+        pa, pb = phase >> 1, phase & 1
+        acc = _F64Acc(split)
+        k0 = 0
+        for si in range(d.nseg):
+            seg = d.segs[si]
+            width = seg.cblocks * 64
+            a = tuple(None if p is None else _gather(p, d.srcs[seg.src], seg.dh + pa, seg.dw + pb, d.Nt, d.Ht, d.Wt, width) for p in srcs[seg.src])
+            acc.add(a, tuple(None if p is None else p[phase * d.Cout:(phase + 1) * d.Cout, k0:k0 + width] for p in w))
+            k0 += width
+        off = 2 * (pa * d.out_pitch_h + pb * d.out_pitch_w)
+        strides = (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1)
+        _f64_emit(d, acc, float(d.acc_scale) if d.acc_scale != 0 else 1.0, (d.out or 0) + off, (d.Nt, d.Ht, d.Wt, d.Cout), strides,
+                  (d.residual + off) if d.residual else None, d.out_plane if split else 0, d.res_plane if split else 0, sink)
+
+
+def _gather(sv, src, dh, dw, Nt, Ht, Wt, width):
+    """A operand of one tap: [Nt, Ht, Wt, width] of the view `sv` [N, H, W, C] shifted by (dh, dw), zero outside the view"""
+    hh = np.arange(Ht)[:, None] + dh
+    ww = np.arange(Wt)[None, :] + dw
+    inb = (hh >= 0) & (hh < src.H) & (ww >= 0) & (ww < src.W)
+    g = sv[:, np.clip(hh, 0, src.H - 1), np.clip(ww, 0, src.W - 1), :min(width, sv.shape[-1])] * inb[None, :, :, None]
+    a = np.zeros((Nt, Ht, Wt, width), dtype=sv.dtype)
+    nn = min(Nt, src.N)
+    a[:nn, :, :, :g.shape[-1]] = g[:nn]
+    return a
+
+
 def run_desc(d, sink=None):
     """Execute descriptor `d` (host pointers) and write its outputs like the device kernel would.
     Split descriptors: operands are hi + lo pairs; the contraction is done in float64 (the kernel's fp32 accumulation of
     hi*hi + hi*lo + lo*hi differs from it by ~1e-7 relative), the epilogue in fp32 exactly like the kernel.
-    sink (fast mode-0 descriptors only): float64 reference mode. Nothing is written; for every output phase
-    sink(ptr, shape, strides, value, magnitude) receives the exact float64 result (+ residual, ReLU) of the fp16 operands and
-    the same contraction over |x|*|w| (+ |residual|), which scales the accumulation error of the kernel."""
+    sink: float64 reference mode, both precisions and both modes. Nothing is written; for every output phase
+    sink(ptr, shape, strides, value, mag, parts, plane) receives the exact float64 result of the operands' values and the
+    magnitudes that scale the kernel's error (see _F64Acc and _f64_emit)."""
+    if sink is not None:
+        return _run_desc_f64(d, sink)
     split = bool(d.split)
-    f64 = sink is not None
-    assert not (f64 and (split or d.mode != 0)), "the float64 reference mode covers fast mode-0 descriptors"
     K = 64 * sum(d.segs[i].cblocks for i in range(d.nseg))
     rows = d.phases * d.Cout
     wts = _pair(d.weights, rows * K if split else 0, (rows, K), (K, 1))
-    if not split and not f64:
+    if not split:
         wts = wts.astype(np.float32)
     scale = np.float32(d.acc_scale if d.acc_scale != 0 else 1.0)
     bias = _view(d.bias, (d.Cout,), (1,), np.float32) if d.bias else None
     Nt, Ht, Wt = d.Nt, d.Ht, d.Wt
-    hh0 = np.arange(Ht)[:, None]
-    ww0 = np.arange(Wt)[None, :]
-    acc_t = np.float64 if (split or f64) else np.float32
+    acc_t = np.float64 if split else np.float32
     for phase in range(d.phases):
         pa, pb = phase >> 1, phase & 1
         acc = np.zeros((Nt, Ht, Wt, d.Cout), dtype=acc_t)
-        mag = np.zeros_like(acc) if f64 else None
         k0 = 0
         for si in range(d.nseg):
             seg = d.segs[si]
             src = d.srcs[seg.src]
             width = seg.cblocks * 64
             sv = _pair(src.ptr, src.plane if split else 0, (src.N, src.H, src.W, min(width, src.C)), (src.pitch_n, src.pitch_h, src.pitch_w, 1))
-            hh = hh0 + seg.dh + pa
-            ww = ww0 + seg.dw + pb
-            inb = (hh >= 0) & (hh < src.H) & (ww >= 0) & (ww < src.W)
-            a = np.zeros((Nt, Ht, Wt, width), dtype=acc_t)
-            g = sv[:, np.clip(hh, 0, src.H - 1), np.clip(ww, 0, src.W - 1), :].astype(acc_t)  # [N, Ht, Wt, c]
-            g = g * inb[None, :, :, None]
-            nn = min(Nt, src.N)
-            a[:nn, :, :, :g.shape[-1]] = g[:nn]
-            wseg = wts[phase * d.Cout:(phase + 1) * d.Cout, k0:k0 + width]
-            acc += np.tensordot(a, wseg, axes=([3], [1]))
-            if f64:
-                mag += np.tensordot(np.abs(a), np.abs(wseg), axes=([3], [1]))
+            a = _gather(sv.astype(acc_t), src, seg.dh + pa, seg.dw + pb, Nt, Ht, Wt, width)
+            acc += np.tensordot(a, wts[phase * d.Cout:(phase + 1) * d.Cout, k0:k0 + width], axes=([3], [1]))
             k0 += width
-        if f64:
-            base = d.out + 2 * (pa * d.out_pitch_h + pb * d.out_pitch_w)
-            shape = (Nt, Ht, Wt, d.Cout)
-            strides = (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1)
-            acc *= float(scale)
-            mag *= float(scale)
-            if bias is not None:
-                acc += bias
-                mag += np.abs(bias)
-            if d.residual:
-                r = _view(d.residual + 2 * (pa * d.out_pitch_h + pb * d.out_pitch_w), shape, strides).astype(np.float64)
-                acc += r
-                mag += np.abs(r)
-            sink(base, shape, strides, np.maximum(acc, 0) if d.relu else acc, mag)
-            continue
         acc = acc.astype(np.float32) * scale
         if bias is not None:
             acc += bias
@@ -147,11 +225,29 @@ def run_desc(d, sink=None):
             ov[...] = np.transpose(logits, (0, 3, 1, 2))
 
 
-def run_rowdesc(d):
-    """CPU semantics of rsb_rowconv_run (line-buffer kernel): same arithmetic as run_desc, described by taps instead of segments"""
+def run_rowdesc(d, sink=None):
+    """CPU semantics of rsb_rowconv_run (line-buffer kernel): same arithmetic as run_desc, described by taps instead of segments.
+    sink: the float64 reference mode of run_desc."""
     nph = d.nphase_a * d.nsub
     K = d.taps_h * d.taps_w * d.cin
     split = bool(getattr(d, "split", 0))
+    if sink is not None:
+        w = _operand(d.weights, nph * d.Cout * K if split else 0, (nph * d.Cout, K), (K, 1))
+        s = d.src
+        sv = _operand(s.ptr, s.plane if split else 0, (s.N, s.H, s.W, d.cin), (s.pitch_n, s.pitch_h, s.pitch_w, 1))
+        strides = (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1)
+        for a in range(d.nphase_a):
+            for s_ in range(d.nsub):
+                acc = _F64Acc(split)
+                r0 = (a * d.nsub + s_) * d.Cout
+                for th in range(d.taps_h):
+                    for tw in range(d.taps_w):
+                        k0 = (th * d.taps_w + tw) * d.cin
+                        acc.add(tuple(None if p is None else _gather(p, s, d.dh0 + a + th, d.dw0 + s_ + tw, d.Nt, d.Ht, d.Wt, d.cin) for p in sv),
+                                tuple(None if p is None else p[r0:r0 + d.Cout, k0:k0 + d.cin] for p in w))
+                _f64_emit(d, acc, float(d.acc_scale) if split and d.acc_scale != 0 else 1.0,
+                          (d.out or 0) + 2 * (a * d.out_pitch_h + s_ * d.out_pitch_w), (d.Nt, d.Ht, d.Wt, d.Cout), strides, None, 0, 0, sink)
+        return
     wts = _pair(d.weights, nph * d.Cout * K if split else 0, (nph * d.Cout, K), (K, 1))
     if not split:
         wts = wts.astype(np.float32)
@@ -192,12 +288,18 @@ def run_rowdesc(d):
 
 def run_engine(engine, x):
     """Execute a plan_only UNetEngine (CPU buffers) op by op; returns fp32 NCHW logits (torch)."""
+    run_engine_ops(engine, engine.ops, x)
+    return engine.logits.clone()
+
+
+def run_engine_ops(engine, ops, x):
+    """Execute `ops` (entries of engine.ops) of a plan_only UNetEngine; x: fp32 NCHW normalised input (CPU), read by the pre-pass."""
     import torch
     import torch.nn.functional as F
 
     assert engine.plan_only and engine.device.type == "cpu"
     strict = getattr(engine, "strict", False)
-    for op in engine.ops:
+    for op in ops:
         if op[0] == "prepass":
             engine.s2d.copy_(prepass_s2d_split_cpu(x) if strict else prepass_s2d_cpu(x))
         elif op[0] == "maxpool":
@@ -214,7 +316,6 @@ def run_engine(engine, x):
             run_rowdesc(op[1].desc)
         else:
             run_desc(op[1].desc)
-    return engine.logits.clone()
 
 
 # --------------------------------------------------------------------------------------------------
@@ -226,14 +327,7 @@ def _gather_segment(d, seg, phase, dtype=np.float32):
     src = d.srcs[seg.src]
     width = seg.cblocks * 64
     sv = _view(src.ptr, (src.N, src.H, src.W, min(width, src.C)), (src.pitch_n, src.pitch_h, src.pitch_w, 1))
-    hh = np.arange(d.Ht)[:, None] + seg.dh + pa
-    ww = np.arange(d.Wt)[None, :] + seg.dw + pb
-    inb = (hh >= 0) & (hh < src.H) & (ww >= 0) & (ww < src.W)
-    g = sv[:, np.clip(hh, 0, src.H - 1), np.clip(ww, 0, src.W - 1), :].astype(dtype) * inb[None, :, :, None]
-    a = np.zeros((d.Nt, d.Ht, d.Wt, width), dtype=dtype)
-    nn = min(d.Nt, src.N)
-    a[:nn, :, :, :g.shape[-1]] = g[:nn]
-    return a
+    return _gather(sv, src, seg.dh + pa, seg.dw + pb, d.Nt, d.Ht, d.Wt, width).astype(dtype)
 
 
 def run_wgrad(d, dy_ptr, dw, f64=False):

@@ -124,13 +124,18 @@ class GpuExecutor:
 
 
 class _Write:
-    """an output view (base buffer index, element offset, shape, element strides) with its reference and tolerance"""
+    """an output view (base buffer index, element offset, shape, element strides) with its reference and tolerance.
+    plane > 0: the output is an fp16 (hi, lo) pair whose lo plane lies `plane` elements behind the hi plane; the value
+    compared with the reference is hi + lo."""
 
-    __slots__ = ("label", "idx", "off", "shape", "strides", "ref", "tol", "tag")
+    __slots__ = ("label", "idx", "off", "shape", "strides", "ref", "tol", "tag", "plane")
 
-    def __init__(self, label, idx, off, shape, strides, ref, tol, tag):
+    def __init__(self, label, idx, off, shape, strides, ref, tol, tag, plane=0):
         self.label, self.idx, self.off, self.shape, self.strides = label, idx, off, tuple(shape), tuple(strides)
-        self.ref, self.tol, self.tag = ref, tol, tag
+        self.ref, self.tol, self.tag, self.plane = ref, tol, tag, plane
+
+    def offsets(self):
+        return (self.off, self.off + self.plane) if self.plane else (self.off,)
 
 
 def _bases(eng):
@@ -146,7 +151,136 @@ def _bits(t):
     return t.view({2: torch.int16, 4: torch.int32, 8: torch.int64}[t.element_size()]) if t.dtype.is_floating_point else t
 
 
-class Lockstep:
+def _same(a, b):
+    """bit equality of two tensors of one shape and dtype (on the CPU as 8-byte words: torch.equal there is ~10x slower)"""
+    if a.device.type != "cpu":
+        return torch.equal(_bits(a), _bits(b))
+    x, y = a.reshape(-1).view(torch.uint8).numpy(), b.reshape(-1).view(torch.uint8).numpy()
+    n = x.size - x.size % 8
+    return np.array_equal(x[:n].view(np.int64), y[:n].view(np.int64)) and np.array_equal(x[n:], y[n:])
+
+
+class Harness:
+    """What the training and the inference lockstep checks share: buffers of the executor under test (`db`) and of the CPU
+    twin (`tb`) paired by position, pointer -> (buffer, offset) lookup in the twin, the stray-write check on the executor's
+    device, the elementwise comparison with teacher forcing, and the report. The twin's elements map to the executor's
+    one to one here; a subclass that replays a subset of the executor's batch overrides _dut_view / _dut_mark / _pull."""
+
+    def _index(self):
+        self._order = sorted((t.data_ptr(), i) for i, t in enumerate(self.tb) if t.numel())
+        self._starts = [p for p, _ in self._order]
+
+    # ------------------------------------------------------------------ addressing
+    def _locate(self, ptr):
+        k = bisect.bisect_right(self._starts, ptr) - 1
+        assert k >= 0, "pointer outside every buffer"
+        p, i = self._order[k]
+        t = self.tb[i]
+        assert ptr < p + t.numel() * t.element_size(), "pointer outside every buffer"
+        assert (ptr - p) % t.element_size() == 0
+        return i, (ptr - p) // t.element_size()
+
+    def _label(self, t, name):
+        i, off = self._locate(t.data_ptr())
+        if off == 0 and t.numel() == self.tb[i].numel():
+            self.labels.setdefault(i, name)
+
+    def _blabel(self, i):
+        return self.labels.get(i, "buffer#%d %s%s" % (i, self.tb[i].dtype, tuple(self.tb[i].shape)))
+
+    def _write_t(self, label, t, ref, tol, tag):
+        """output = the whole of (twin) tensor `t`"""
+        i, off = self._locate(t.data_ptr())
+        tol = np.asarray(tol)
+        return _Write(label, i, off, t.shape, t.stride(), np.asarray(ref).reshape(t.shape), tol.reshape(t.shape) if tol.ndim else tol, tag)
+
+    def _dut_view(self, b, off, shape, strides):
+        """the executor's elements that twin view (buffer b, off, shape, strides) stands for, same shape"""
+        return _view(self.db[b], off, shape, strides)
+
+    def _dut_mark(self, mask, b, off, shape, strides):
+        """mark in `mask` (flat bool, executor buffer b's size and device) every element the op may write for that twin view"""
+        torch.as_strided(mask, shape, strides, off).fill_(True)
+
+    def _pull(self, b):
+        """executor buffer b as the twin holds it, on the CPU"""
+        return self.db[b].cpu()
+
+    def _fail(self, which, i, ot, buffer, msg):
+        text = "%s op %d (%s %s), buffer %s: %s" % (which, i, ot[0], self._name(ot), buffer, msg)
+        err = LockstepError(text, i, which, ot[0], self._name(ot), buffer)
+        if self.raise_on_fail:
+            raise err
+        self.failures.append(err)
+
+    def _check_stray(self, which, i, ot, writes):
+        by_base = {}
+        for w in writes:
+            by_base.setdefault(w.idx, []).append(w)
+        for b in self.tracked:
+            cur, snap = self.db[b], self.snap[b]
+            if b not in by_base:
+                if _same(cur, snap):
+                    continue
+                changed = (_bits(cur) != _bits(snap)).reshape(-1)
+            else:
+                mask = torch.zeros(cur.numel(), dtype=torch.bool, device=cur.device)
+                for w in by_base[b]:
+                    for off in w.offsets():
+                        self._dut_mark(mask, b, off, w.shape, w.strides)
+                changed = (_bits(cur) != _bits(snap)).reshape(-1) & ~mask
+                if not bool(changed.any()):
+                    snap.copy_(cur)
+                    continue
+            first = int(torch.nonzero(changed)[0])
+            n = int(changed.sum())
+            pos = np.unravel_index(first, tuple(cur.shape)) if cur.dim() else ()
+            self._fail(which, i, ot, self._blabel(b), "%d stray write(s) outside the op's outputs, first at %s" % (n, tuple(int(v) for v in pos)))
+            snap.copy_(cur)
+            self.tb[b].copy_(self._pull(b))  # the twin follows, so later ops are checked on what the executor really holds
+
+    def _compare(self, which, i, ot, w):
+        got_t = [self._dut_view(w.idx, off, w.shape, w.strides).cpu() for off in w.offsets()]
+        got = sum(t.double() for t in got_t).numpy()
+        ref = np.asarray(w.ref, dtype=np.float64)
+        tol = np.broadcast_to(np.asarray(w.tol, dtype=np.float64), ref.shape)
+        err = np.abs(got - ref)
+        err = np.where(np.isnan(err) & ~(np.isnan(got) & np.isnan(ref)), np.inf, err)
+        err = np.where(np.isnan(err), 0.0, err)
+        exact = not np.any(tol)
+        st = self.stats.setdefault(w.tag, [0, 0.0, exact])
+        st[0] += 1
+        st[2] = st[2] and exact
+        if exact:
+            worst = float(err.max()) if err.size else 0.0
+            st[1] = max(st[1], worst)
+            bad = err > 0
+        else:
+            ratio = np.divide(err, tol, out=np.where(err > 0, np.inf, 0.0), where=tol > 0)
+            st[1] = max(st[1], float(ratio.max()) if ratio.size else 0.0)
+            bad = err > tol
+        if w.tag == "bn_apply":
+            self.bn_apply_elems += got.size
+            self.ulp_flips += int((got != ref.astype(np.float16).astype(np.float64)).sum())
+        if bad.any():
+            k = int(np.argmax(np.where(bad, err / np.maximum(tol, 1e-300), -1)))
+            pos = np.unravel_index(k, ref.shape)
+            self._fail(which, i, ot, w.label, "%d element(s) out of tolerance; worst at %s: got %r, float64 reference %r, tolerance %r" % (
+                int(bad.sum()), tuple(int(v) for v in pos), float(got.reshape(-1)[k]), float(ref.reshape(-1)[k]), float(tol.reshape(-1)[k])))
+        for off, t in zip(w.offsets(), got_t):
+            _view(self.tb[w.idx], off, w.shape, w.strides).copy_(t)
+
+    def table(self):
+        lines = ["%-22s %7s  %s" % ("kind", "checks", "worst err/tol (exact kinds: worst |err|)")]
+        for tag in sorted(self.stats):
+            n, worst, exact = self.stats[tag]
+            lines.append("%-22s %7d  %s" % (tag, n, ("exact, max |err| %g" % worst) if exact else "%.3g" % worst))
+        return "\n".join(lines + self._table_extra())
+
+
+class Lockstep(Harness):
+    """the training plan: fwd_ops then bwd_ops of a UNetTrainEngine"""
+
     def __init__(self, dut, twin):
         self.dut, self.tw = dut, twin
         E, T = dut.eng, twin
@@ -158,8 +292,7 @@ class Lockstep:
         for which in ("fwd_ops", "bwd_ops"):
             a, b = getattr(E, which), getattr(T, which)
             assert [o[0] for o in a] == [o[0] for o in b], "the two engines built different %s" % which
-        self._order = sorted((t.data_ptr(), i) for i, t in enumerate(self.tb) if t.numel())
-        self._starts = [p for p, _ in self._order]
+        self._index()
         # labels of the base buffers, for messages
         self.labels = {}
         for name, t in list(T.params.items()):
@@ -200,29 +333,12 @@ class Lockstep:
         self.failures = []
         self.checked = {"fwd": set(), "bwd": set()}
 
-    # ------------------------------------------------------------------ addressing
-    def _locate(self, ptr):
-        k = bisect.bisect_right(self._starts, ptr) - 1
-        assert k >= 0, "pointer outside every buffer"
-        p, i = self._order[k]
-        t = self.tb[i]
-        assert ptr < p + t.numel() * t.element_size(), "pointer outside every buffer"
-        assert (ptr - p) % t.element_size() == 0
-        return i, (ptr - p) // t.element_size()
-
-    def _label(self, t, name):
-        i, off = self._locate(t.data_ptr())
-        if off == 0 and t.numel() == self.tb[i].numel():
-            self.labels.setdefault(i, name)
-
-    def _blabel(self, i):
-        return self.labels.get(i, "buffer#%d %s%s" % (i, self.tb[i].dtype, tuple(self.tb[i].shape)))
-
-    def _write_t(self, label, t, ref, tol, tag):
-        """output = the whole of (twin) tensor `t`"""
-        i, off = self._locate(t.data_ptr())
-        tol = np.asarray(tol)
-        return _Write(label, i, off, t.shape, t.stride(), np.asarray(ref).reshape(t.shape), tol.reshape(t.shape) if tol.ndim else tol, tag)
+    def _table_extra(self):
+        lines = []
+        if self.bn_apply_elems:
+            lines.append("bn_apply outputs one fp16 ulp from the correctly rounded value: %d of %d" % (self.ulp_flips, self.bn_apply_elems))
+        lines.append("ops checked: %d forward, %d backward" % (len(self.checked["fwd"]), len(self.checked["bwd"])))
+        return lines
 
     # ------------------------------------------------------------------ driver
     def run(self, x, dlogits, raise_on_fail=True, dut_x=None, dut_dlogits=None):
@@ -252,13 +368,6 @@ class Lockstep:
             return ot[1].name
         return k
 
-    def _fail(self, which, i, ot, buffer, msg):
-        text = "%s op %d (%s %s), buffer %s: %s" % (which, i, ot[0], self._name(ot), buffer, msg)
-        err = LockstepError(text, i, which, ot[0], self._name(ot), buffer)
-        if self.raise_on_fail:
-            raise err
-        self.failures.append(err)
-
     def _step(self, which, i, od, ot, fin, x, dlogits, dx, ddl):
         writes = self._reference(ot, x, dlogits)
         self.dut.run(od, x=dx, dlogits=ddl)
@@ -278,61 +387,6 @@ class Lockstep:
         self._extra(which, i, ot)
 
     # ------------------------------------------------------------------ invariants
-    def _check_stray(self, which, i, ot, writes):
-        by_base = {}
-        for w in writes:
-            by_base.setdefault(w.idx, []).append(w)
-        for b in self.tracked:
-            cur, snap = self.db[b], self.snap[b]
-            if b not in by_base:
-                if torch.equal(_bits(cur), _bits(snap)):
-                    continue
-                changed = (_bits(cur) != _bits(snap)).reshape(-1)
-            else:
-                mask = torch.zeros(cur.numel(), dtype=torch.bool, device=cur.device)
-                for w in by_base[b]:
-                    torch.as_strided(mask, w.shape, w.strides, w.off).fill_(True)
-                changed = (_bits(cur) != _bits(snap)).reshape(-1) & ~mask
-                if not bool(changed.any()):
-                    snap.copy_(cur)
-                    continue
-            first = int(torch.nonzero(changed)[0])
-            n = int(changed.sum())
-            pos = np.unravel_index(first, tuple(cur.shape)) if cur.dim() else ()
-            self._fail(which, i, ot, self._blabel(b), "%d stray write(s) outside the op's outputs, first at %s" % (n, tuple(int(v) for v in pos)))
-            snap.copy_(cur)
-            self.tb[b].copy_(cur.cpu())  # the twin follows, so later ops are checked on what the executor really holds
-
-    def _compare(self, which, i, ot, w):
-        got_t = _view(self.db[w.idx], w.off, w.shape, w.strides).cpu()
-        got = got_t.double().numpy()
-        ref = np.asarray(w.ref, dtype=np.float64)
-        tol = np.broadcast_to(np.asarray(w.tol, dtype=np.float64), ref.shape)
-        err = np.abs(got - ref)
-        err = np.where(np.isnan(err) & ~(np.isnan(got) & np.isnan(ref)), np.inf, err)
-        err = np.where(np.isnan(err), 0.0, err)
-        exact = not np.any(tol)
-        st = self.stats.setdefault(w.tag, [0, 0.0, exact])
-        st[0] += 1
-        st[2] = st[2] and exact
-        if exact:
-            worst = float(err.max()) if err.size else 0.0
-            st[1] = max(st[1], worst)
-            bad = err > 0
-        else:
-            ratio = np.divide(err, tol, out=np.where(err > 0, np.inf, 0.0), where=tol > 0)
-            st[1] = max(st[1], float(ratio.max()) if ratio.size else 0.0)
-            bad = err > tol
-        if w.tag == "bn_apply":
-            self.bn_apply_elems += got.size
-            self.ulp_flips += int((got != ref.astype(np.float16).astype(np.float64)).sum())
-        if bad.any():
-            k = int(np.argmax(np.where(bad, err / np.maximum(tol, 1e-300), -1)))
-            pos = np.unravel_index(k, ref.shape)
-            self._fail(which, i, ot, w.label, "%d element(s) out of tolerance; worst at %s: got %r, float64 reference %r, tolerance %r" % (
-                int(bad.sum()), tuple(int(v) for v in pos), float(got.reshape(-1)[k]), float(ref.reshape(-1)[k]), float(tol.reshape(-1)[k])))
-        _view(self.tb[w.idx], w.off, w.shape, w.strides).copy_(got_t)
-
     def _extra(self, which, i, ot):
         k = ot[0]
         if k == "conv":
@@ -372,7 +426,7 @@ class Lockstep:
         K = 64 * sum(d.segs[j].cblocks for j in range(d.nseg))
         writes = []
 
-        def sink(ptr, shape, strides, val, mag):
+        def sink(ptr, shape, strides, val, mag, parts, plane):
             idx, off = self._locate(ptr)
             tag = "conv.dgrad" if ".dgrad" in op[1].name else "conv"
             writes.append(_Write("%s out (%s)" % (op[1].name, self._blabel(idx)), idx, off, shape, strides, val, ulp16(val) + K * U * mag, tag))
@@ -555,16 +609,6 @@ class Lockstep:
                 self._write_t("final.weight grad", T.grads["final.weight"], dw, E_SUM * dwm + 2 * U * np.abs(dw), "final_bwd.dw_db"),
                 self._write_t("final.bias grad", T.grads["final.bias"], db, E_SUM * dbm + 2 * U * np.abs(db), "final_bwd.dw_db")]
 
-    # ------------------------------------------------------------------ report
-    def table(self):
-        lines = ["%-22s %7s  %s" % ("kind", "checks", "worst err/tol (exact kinds: worst |err|)")]
-        for tag in sorted(self.stats):
-            n, worst, exact = self.stats[tag]
-            lines.append("%-22s %7d  %s" % (tag, n, ("exact, max |err| %g" % worst) if exact else "%.3g" % worst))
-        if self.bn_apply_elems:
-            lines.append("bn_apply outputs one fp16 ulp from the correctly rounded value: %d of %d" % (self.ulp_flips, self.bn_apply_elems))
-        lines.append("ops checked: %d forward, %d backward" % (len(self.checked["fwd"]), len(self.checked["bwd"])))
-        return "\n".join(lines)
 
 
 def make_pair(C, B, H, W, loss_scale, device, seed=0):

@@ -68,6 +68,27 @@ def test_encode_p8_round_trips_through_pil(level, tmp_path):
         assert im.getpalette()[:768] == pal  # what `rs masks` / a viewer reads back is what predict.py:105-108 would have written
 
 
+def test_save_batch_writes_each_callers_palette(tmp_path):
+    """tools/predict.py's writers get a fresh palette list per call (`rs rasterize` after `rs predict` in one process): each
+    file carries the palette it was written with, even when a new list takes the address of a freed one"""
+    from robosat_b200.tools.predict import _save_batch, _save_png
+
+    q = np.zeros((2, 8, 8), np.uint8)
+    q[:, 2:5, 3:6] = 1
+    cases = [("pink", None), ("denim", "orange"), ("pink", None), ("dark", "gray"), ("denim", "orange"), ("teal", "red")] * 3
+    for i, (a, b) in enumerate(cases):
+        want = colors.continuous_palette_for_color(a, 256) if b is None else colors.make_palette(a, b)
+        if i % 2:
+            _save_batch(str(tmp_path), list(want), [(i, 0, 1), (i, 1, 1)], q, 2)
+        else:
+            for y in range(2):
+                _save_png(str(tmp_path), list(want), i, y, 1, q[y])
+        for y in range(2):
+            im = Image.open(str(tmp_path / "1" / str(i) / ("%d.png" % y)))
+            assert im.getpalette()[:len(want)] == want, (i, a, b)
+            assert np.array_equal(np.asarray(im), q[y])
+
+
 def test_encode_strategy_follows_the_content(tmp_path):
     """noise-like masks skip deflate's string matcher (Z_RLE) without growing; compressible masks keep the default strategy"""
     import os

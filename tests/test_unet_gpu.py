@@ -155,6 +155,38 @@ def test_full_size_batch_properties_512(precision, cuda_device):
     _check(sub.float().cpu(), ref, "512 subset", precision)
 
 
+def test_serve_plan_strict_1x512_matches_oracle(cuda_device):
+    """the measured batch-1 strict plan (`rs serve`, SegmentEngine) end to end against the oracle"""
+    from robosat_b200.engine import plan_table
+
+    assert "strict:1x512x512" in plan_table()
+    sd = synth.make_state_dict(2, seed=0)
+    x = synth.normalize_tiles(synth.make_tiles_u8(1, 512, seed=5))
+    eng = UNetEngine(sd, 2, 1, 512, 512, device=cuda_device, precision="strict")
+    got = eng.forward(x.to(cuda_device)).float().cpu()
+    with torch.no_grad():
+        ref = unet_oracle.unet_forward(sd, x)
+    _check(got, ref, "serve 1x512", "strict")
+
+
+@pytest.mark.parametrize("precision", ["strict", "fast"])
+def test_predict_plan_32x576_matches_oracle(precision, cuda_device):
+    """the measured batch-32 plan of `rs predict --tile_size 512` (576 = 512 + 2 x 32 overlap): two tiles of the batch,
+    one of them the last (a ragged batch tile), against the oracle"""
+    from robosat_b200.engine import plan_table
+
+    assert "%s:32x576x576" % precision in plan_table()
+    sd = synth.make_state_dict(2, seed=0)
+    u8 = synth.make_tiles_u8(32, 576, seed=6)
+    eng = UNetEngine(sd, 2, 32, 576, 576, device=cuda_device, precision=precision)
+    got = eng.forward(u8.to(cuda_device)).float().cpu()
+    del eng
+    pick = [9, 31]
+    with torch.no_grad():
+        ref = unet_oracle.unet_forward(sd, synth.normalize_tiles(u8[pick]))
+    _check(got[pick], ref, "predict 32x576 tiles %s" % pick, precision)
+
+
 def test_six_class_1024_forward(cuda_device):
     """BASELINE config 5 shape: 6 classes, 3x1024x1024 (one tile against the oracle; the batch-8 plan must fit and replay)"""
     sd = synth.make_state_dict(6, seed=0)
