@@ -317,7 +317,8 @@ int rsb_cover_polygons(const double* vertices, const int64_t* ring_offsets, cons
  * order, into keys [capacity] (status[0] of the burn is the number written; status[2] is reset and used as the cursor). */
 int rsb_cover_emit_keys(const uint32_t* bitmap, int64_t bitmap_words, const int64_t* bitmap_offsets, const int64_t* grids, int32_t F,
                         int32_t zoom, int64_t* keys, int64_t capacity, int64_t* status, void* stream);
-/* Ascending sort of n non-negative int64 keys below 2^key_bits (an LSD radix sort of ceil(key_bits / 8) 8-bit passes) and
+/* Ascending sort of n non-negative int64 keys below 2^key_bits (an LSD radix sort of ceil(key_bits / 8) 8-bit passes; key_bits = 64
+ * sorts the whole word as unsigned; bits at or above key_bits are not looked at, so keys that have them come out unsorted) and
  * removal of adjacent duplicates: keys[0 .. *unique_count) holds the result, in place. workspace: DEVICE bytes, at least
  * rsb_sort_unique_workspace_bytes(n). Does not synchronise. */
 int64_t rsb_sort_unique_workspace_bytes(int64_t n);
@@ -551,7 +552,8 @@ int rsb_adam_step(float* param, const float* grad, float* exp_avg, float* exp_av
 /* Same update behind an overflow guard for mixed-precision training (no host synchronisation): if `grad` holds an inf / NaN the
  * whole step is skipped on the device (parameters and moments untouched). guard_state: int32[4] on the device, zero-initialised by
  * the caller once -- [0] scratch flag, [1] steps skipped so far (bias corrections use step - skipped), [2] flag of the last
- * finished step (poll it to adapt the loss scale), [3] steps seen. With no skipped step the result equals rsb_adam_step bit for bit. */
+ * finished step (poll it to adapt the loss scale), [3] steps seen. With no skipped step the result equals rsb_adam_step's to the last bit
+ * of each value (the two kernels' updates are contracted into fused multiply-adds differently). */
 int rsb_adam_step_guarded(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float lr, float b1,
                           float b2, float eps, int32_t step, int32_t* guard_state, void* stream);
 

@@ -26,6 +26,11 @@ __device__ __forceinline__ int warp_sum_i(int v) {
     return v;
 }
 
+// A label outside [0, C) (a stray palette index in a label PNG) must never become an index: weight[t] and logits[t * HW] would read
+// out of bounds. Such a pixel is left out of every sum and gets a zero gradient, as if the image did not contain it. `rs train`
+// rejects these labels on the host (tools/train.py: check_mask_range), so this is the second line of defence, not the report.
+__device__ __forceinline__ bool target_in_range(int64_t t, int C) { return t >= 0 && t < static_cast<int64_t>(C); }
+
 // =================================================================================================
 // CrossEntropyLoss2d (losses.py:24-25): NLLLoss(weight)(log_softmax(x, dim=1), t), reduction = weighted mean
 // =================================================================================================
@@ -34,6 +39,7 @@ __global__ void ce_reduce_kernel(const float* __restrict__ logits, const int64_t
     const int64_t total = static_cast<int64_t>(N) * HW;
     double num = 0.0, den = 0.0;
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        if (!target_in_range(targets[i], C)) continue;
         const int64_t n = i / HW, pix = i % HW;
         const float* l = logits + n * C * HW + pix;
         float m = l[0];
@@ -66,6 +72,10 @@ __global__ void ce_finish_kernel(const float* __restrict__ logits, const int64_t
         const int64_t n = i / HW, pix = i % HW;
         const float* l = logits + n * C * HW + pix;
         float* g = grad + n * C * HW + pix;
+        if (!target_in_range(targets[i], C)) {
+            for (int c = 0; c < C; ++c) g[c * HW] = 0.0f;
+            continue;
+        }
         float m = l[0];
         for (int c = 1; c < C; ++c) m = fmaxf(m, l[c * HW]);
         float s = 0.f;
@@ -88,6 +98,7 @@ __global__ void focal_reduce_kernel(const float* __restrict__ logits, const int6
     const int64_t total = static_cast<int64_t>(N) * HW;
     double num = 0.0, den = 0.0;
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        if (!target_in_range(targets[i], C)) continue;
         const int64_t n = i / HW, pix = i % HW;
         const float* l = logits + n * C * HW + pix;
         float m = l[0];
@@ -121,6 +132,10 @@ __global__ void focal_finish_kernel(const float* __restrict__ logits, const int6
         const int64_t n = i / HW, pix = i % HW;
         const float* l = logits + n * C * HW + pix;
         float* g = grad + n * C * HW + pix;
+        if (!target_in_range(targets[i], C)) {
+            for (int c = 0; c < C; ++c) g[c * HW] = 0.0f;
+            continue;
+        }
         float m = l[0];
         for (int c = 1; c < C; ++c) m = fmaxf(m, l[c * HW]);
         float s = 0.f;
@@ -131,7 +146,9 @@ __global__ void focal_finish_kernel(const float* __restrict__ logits, const int6
         const float q = 1.0f - pt;
         // gamma == 0: the penalty is the constant 1 and its derivative term is zero, as in torch's pow backward (exponent 0
         // gives a zero gradient). Evaluated, it would be 0 * powf(0, -1) = 0 * inf = NaN wherever softmax saturates to p_t = 1.
-        const float dpen = gamma == 0.0f ? 0.0f : gamma * powf(q, gamma - 1.0f) * pt * logp;
+        // q == 0 (softmax saturated at the target, so log p_t == 0 too): the term's limit is 0 for every gamma > 0, since
+        // q^(gamma-1) log p_t ~ -q^gamma. Evaluated for gamma < 1 it is inf * 0 = NaN.
+        const float dpen = (gamma == 0.0f || q == 0.0f) ? 0.0f : gamma * powf(q, gamma - 1.0f) * pt * logp;
         const float k = powf(q, gamma) - dpen;
         const float w = -(weight ? weight[t] : 1.0f) * inv_den * k;
         for (int c = 0; c < C; ++c) {
@@ -155,6 +172,7 @@ __global__ void miou_reduce_kernel(const float* __restrict__ logits, const int64
     __syncthreads();
     double num = 0.0, den = 0.0;
     for (int64_t pix = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; pix < HW; pix += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        if (!target_in_range(targets[static_cast<int64_t>(n) * HW + pix], C)) continue;  // in neither the soft IoU sums nor the cross entropy
         const float* l = logits + static_cast<int64_t>(n) * C * HW + pix;
         float m = l[0];
         for (int c = 1; c < C; ++c) m = fmaxf(m, l[c * HW]);
@@ -209,6 +227,10 @@ __global__ void miou_grad_kernel(const float* __restrict__ logits, const int64_t
         const int64_t n = i / HW, pix = i % HW;
         const float* l = logits + n * C * HW + pix;
         float* g = grad + n * C * HW + pix;
+        if (!target_in_range(targets[i], C)) {
+            for (int c = 0; c < C; ++c) g[c * HW] = 0.0f;
+            continue;
+        }
         float m = l[0];
         for (int c = 1; c < C; ++c) m = fmaxf(m, l[c * HW]);
         float s = 0.f;
@@ -219,15 +241,17 @@ __global__ void miou_grad_kernel(const float* __restrict__ logits, const int64_t
             for (int c = 0; c < C; ++c) g[c * HW] = w * (expf(l[c * HW] - m) / s - (c == t ? 1.0f : 0.0f));
         } else {
             // d miou / d s_c = -(1/CN) * [ m_c / U - I (1 - m_c) / U^2 ];  dx_k = s_k (ds_k - sum_c ds_c s_c)
+            // I / U^2 as (I / U) / U, like torch's div backward: the union of a class that is absent from the image and has
+            // subnormal probabilities is so small that U * U underflows to 0, and 0 / 0 would put NaN into the whole image
             float dot = 0.f;
             for (int c = 0; c < C; ++c) {
                 const float I = static_cast<float>(sums[(n * C + c) * 2]), U = static_cast<float>(sums[(n * C + c) * 2 + 1]);
-                const float ds = -inv_cn * (c == t ? 1.0f / U : -I / (U * U));
+                const float ds = -inv_cn * (c == t ? 1.0f / U : -(I / U) / U);
                 dot += ds * (expf(l[c * HW] - m) / s);
             }
             for (int c = 0; c < C; ++c) {
                 const float I = static_cast<float>(sums[(n * C + c) * 2]), U = static_cast<float>(sums[(n * C + c) * 2 + 1]);
-                const float ds = -inv_cn * (c == t ? 1.0f / U : -I / (U * U));
+                const float ds = -inv_cn * (c == t ? 1.0f / U : -(I / U) / U);
                 const float p = expf(l[c * HW] - m) / s;
                 g[c * HW] = p * (ds - dot);
             }

@@ -144,6 +144,26 @@ def get_dataset_loaders(model, dataset, workers, rank=0, world=1):
     return train_loader, val_loader
 
 
+def check_mask_range(masks, tiles, num_classes):
+    """Reject a batch whose label masks hold a value outside [0, num_classes), naming the first such tile. Runs on the host batch,
+    where the bytes already are, before the upload: the loss kernels leave such pixels out instead of failing, so a label PNG with
+    a stray palette index would otherwise train on silently (the reference raises "Target ... is out of bounds" there)."""
+    flat = masks.reshape(masks.shape[0], -1)
+    lo, hi = flat.amin(dim=1), flat.amax(dim=1)
+    bad = ((lo < 0) | (hi >= num_classes)).nonzero()
+    if bad.numel() == 0:
+        return
+    i = int(bad[0])
+    name = "sample %d of the batch" % i
+    try:  # the collated [Tile(x=[...], y=[...], z=[...])] of SlippyMapTilesConcatenation
+        tile = tiles[0]
+        name = "tile %d/%d/%d" % (int(tile.z[i]), int(tile.x[i]), int(tile.y[i]))
+    except (AttributeError, IndexError, KeyError, TypeError):
+        pass
+    value = int(hi[i]) if int(hi[i]) >= num_classes else int(lo[i])
+    raise ValueError("label mask of %s holds the value %d, but the dataset has the %d classes 0..%d" % (name, value, num_classes, num_classes - 1))
+
+
 def _epoch(loader, num_classes, device, net, criterion, optimizer=None, world=1, scaler=None):
     """One pass of train() (train.py:163-201) or validate() (train.py:204-238): same bookkeeping, batched metrics."""
     from robosat_b200.dist import allreduce_sum_
@@ -153,7 +173,8 @@ def _epoch(loader, num_classes, device, net, criterion, optimizer=None, world=1,
     metrics = Metrics(range(num_classes))
     net.train() if training else net.eval()
     augmenter = None
-    for images, masks, _tiles in loader:
+    for images, masks, tiles in loader:
+        check_mask_range(masks, tiles, num_classes)
         images = images.to(device, non_blocking=True)
         masks = masks.to(device, non_blocking=True)
         if images.dtype == torch.uint8:

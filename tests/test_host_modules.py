@@ -140,3 +140,35 @@ def test_serve_tool_parser_and_cpu_refusal():
     assert (args.tile_size, args.host, args.port) == (512, "127.0.0.1", 5000) and args.func is serve.main
     with pytest.raises(_lib.RsbError):
         Predictor({"state_dict": {}}, {"common": {"cuda": False}}, {"common": {"classes": ["a", "b"], "colors": ["denim", "orange"]}})
+
+
+def test_train_rejects_label_values_outside_the_classes(tmp_path):
+    """`rs train` checks every batch's masks on the host, before the upload, and names the tile: through the real dataset and
+    DataLoader collation, for the uint8 masks of the device-augment path and the int64 masks of MaskToTensor."""
+    from torch.utils.data import DataLoader
+
+    from robosat_b200.tools.train import _MaskToUint8, check_mask_range
+
+    coords = [(10, 20), (10, 21), (11, 20), (11, 21)]
+    for sub in ("images", "labels"):
+        for x, y in coords:
+            os.makedirs(tmp_path / sub / "18" / str(x), exist_ok=True)
+    for k, (x, y) in enumerate(coords):
+        Image.fromarray(np.zeros((8, 8, 3), np.uint8)).save(tmp_path / "images" / "18" / str(x) / ("%d.png" % y))
+        mask = np.zeros((8, 8), np.uint8)
+        mask[2:5, 2:5] = 1
+        if k == 2:
+            mask[7, 7] = 5  # a stray palette index
+        img = Image.fromarray(mask, mode="P")
+        img.putpalette([0, 0, 0, 255, 255, 255] + [0] * (254 * 3))
+        img.save(tmp_path / "labels" / "18" / str(x) / ("%d.png" % y))
+    for mask_transform in (_MaskToUint8(), MaskToTensor()):
+        transform = JointCompose([JointTransform(ImageToTensor(), mask_transform)])
+        ds = SlippyMapTilesConcatenation([str(tmp_path / "images")], str(tmp_path / "labels"), transform)
+        (images, masks, tiles), = list(DataLoader(ds, batch_size=4, shuffle=False))
+        check_mask_range(masks, tiles, 6)  # 0..5 are all classes of a six-class dataset
+        check_mask_range(masks[:2], tiles, 2)
+        with pytest.raises(ValueError, match=r"tile 18/11/20 holds the value 5, but the dataset has the 2 classes 0\.\.1"):
+            check_mask_range(masks, tiles, 2)
+    with pytest.raises(ValueError, match="sample 1 of the batch holds the value -1"):
+        check_mask_range(torch.tensor([[[0, 1]], [[-1, 0]]]), None, 2)

@@ -41,7 +41,8 @@ def test_lovasz_matches_reference_fixture(tag, cuda_device):
 
 
 def test_lovasz_full_size_against_oracle(cuda_device):
-    """BASELINE config 3 shape per image (2 x 512 x 512), N = 4, ragged tail (P not a multiple of the sort tile is covered by fixture b)."""
+    """BASELINE config 3 shape per image (2 x 512 x 512), N = 4: P is 128 whole sort tiles. Fixture b (P = 1536) is less than one
+    tile; several tiles with a ragged last one, N that is not a power of two and equal errors are in tests/test_losses_edges_gpu.py."""
     g = torch.Generator().manual_seed(5)
     logits = torch.randn((4, 2, 512, 512), generator=g) * 3
     targets = synth.make_masks(4, 512, 2, seed=9)
@@ -91,7 +92,7 @@ def test_adam_matches_reference_fixture(cuda_device):
 
 
 def test_guarded_adam_skips_non_finite_steps_and_equals_plain_adam_otherwise(cuda_device):
-    """rsb_adam_step_guarded: bit-identical to rsb_adam_step while gradients are finite; a step with an inf / NaN gradient leaves
+    """rsb_adam_step_guarded: equal to rsb_adam_step (to the last bit of each value) while gradients are finite; a step with an inf / NaN gradient leaves
     parameters and moments untouched, is counted, and later bias corrections use the number of steps actually taken (what
     torch.optim.Adam behind a GradScaler does)."""
     lib = _lib.load()

@@ -60,6 +60,20 @@ def test_lovasz_oracle_matches_reference():
         np.testing.assert_allclose(grad.numpy(), gold["lovasz_%s_grad" % tag], rtol=0, atol=1e-9)
 
 
+def test_lovasz_oracle_gradient_is_bit_identical_to_the_reference_also_at_n_3():
+    """The GPU tests compare the kernel's gradient with this oracle bit for bit, so the oracle itself has to be bit-identical to the
+    reference. Fixture b has N = 3, where scaling by fp32(1 / N) (autograd of `loss / N`) and dividing by N differ in the last bit."""
+    gold = np.load(os.path.join(GOLD, "losses.npz"))
+    for tag in "abc":
+        logits = torch.from_numpy(gold["lovasz_%s_logits" % tag])
+        targets = torch.from_numpy(gold["lovasz_%s_targets" % tag])
+        grad = losses_oracle.lovasz_loss(logits, targets, with_grad=True)[1].numpy()
+        ref = gold["lovasz_%s_grad" % tag]
+        # every non-zero element has the same bits; where the error is <= 0 autograd leaves -0.0 or +0.0, which compare equal
+        assert np.array_equal(grad, ref) and np.array_equal(grad.view(np.int32)[ref != 0], ref.view(np.int32)[ref != 0]), tag
+    assert gold["lovasz_b_logits"].shape[0] == 3
+
+
 def test_cross_entropy_oracle_matches_reference():
     gold = np.load(os.path.join(GOLD, "losses.npz"))
     for tag in "abc":
