@@ -486,6 +486,22 @@ int rsb_extract_gather(const int64_t* refs, const int32_t* ref_way, int64_t num_
 int rsb_extract_valid(const int32_t* verts, const int64_t* ring_offsets, int32_t R, const int32_t* flags, const int32_t* long_rings, int32_t L,
                       const int64_t* tile_offsets, int32_t* scratch, int32_t* lens, uint8_t* valid, void* stream);
 
+/* `rs compare` (robosat/tools/compare.py; the rule is restated in DESIGN.md §8). Device pointers unless noted.
+ * rsb_compare_count: masks uint8 [N][M] planes of hw bytes, plane (n, m) at masks + (n * M + m) * pitch; labels uint8 [N] planes at
+ * labels + n * pitch, or NULL. counts int64 [N][M][4] = (tp, fp, fn, tn) of mask (n, m) against label n, where "foreground" is
+ * index != 0 in both; without labels the label is taken as all background (tp = fn = 0). The mask's non-zero count, the
+ * numerator of the coverage filter, is tp + fp. pitch % 16 == 0 and 16-byte aligned planes; integer sums, so the counts do not
+ * depend on the launch shape. 1 <= M <= RSB_COMPARE_MAX_PLANES - 1; allocates nothing and does not synchronise. */
+#define RSB_COMPARE_MAX_PLANES 32
+int rsb_compare_count(const uint8_t* masks, const uint8_t* labels, int32_t N, int32_t M, int64_t hw, int64_t pitch, int64_t* counts, void* stream);
+/* rsb_compare_compose: the side-by-side composite image | plane 0 | plane 1 | ... of N tiles of H x W. images uint8 [N][H][W][3]
+ * (image n at images + n * H * W * 3); planes uint8 [N][P] index planes of H * W bytes at planes + (n * P + p) * pitch (plane 0 is
+ * the label, planes 1.. the masks); palettes uint32 [N][P][256] (r | g << 8 | b << 16). out uint8 [N][H][(1 + P) * W][3], tile n
+ * at out + n * out_stride, out_stride % 16 == 0; `out` may be pinned host memory (written through its device mapping) or device
+ * memory. 1 <= P <= RSB_COMPARE_MAX_PLANES - 1; allocates nothing and does not synchronise. */
+int rsb_compare_compose(const uint8_t* images, const uint8_t* planes, const uint32_t* palettes, int32_t N, int32_t P, int32_t H, int32_t W,
+                        int64_t pitch, uint8_t* out, int64_t out_stride, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Host-side PNG codec for the files either side of the predict path (HOST pointers, plain C over zlib, no Python / GIL so the
  * tools' pool threads run truly in parallel). Pixel-identical to PIL; not a compute fallback -- no device work happens here.
@@ -513,6 +529,24 @@ int rsb_png_read_rgb_batch(const char* const* paths, int32_t n, uint8_t* const* 
                            int32_t threads, int32_t* rcs_host);
 int rsb_png_write_p8_batch(const char* const* paths, int32_t n, const uint8_t* pixels_host, int64_t image_stride, int32_t w, int32_t h,
                            const uint8_t* palette_rgb_host, int32_t entries, int32_t level, int32_t threads, int32_t make_dirs);
+
+/* `Image.open(path).convert("P")` of `rs compare` (robosat/tools/compare.py:31-38) for non-interlaced palette PNGs of 1, 2, 4 or 8
+ * bits and 8-bit gray PNGs: out_index_host uint8 [h][w] (the index plane; gray: index = value), out_palette_rgb_host uint8 [256][3]
+ * (the PLTE entries, zero past them; gray: the ramp (i, i, i)), *entries_host = the PLTE entry count (gray: 256). A tRNS chunk is
+ * ignored. RSB_E_UNSUPPORTED for other PNG flavours / non-PNG files (the caller then uses PIL). */
+int rsb_png_decode_indexed(const uint8_t* file_bytes_host, int64_t n, uint8_t* out_index_host, uint8_t* out_palette_rgb_host, int32_t* entries_host,
+                           int32_t w_expected, int32_t h_expected);
+int rsb_png_read_indexed(const char* path, uint8_t* out_index_host, uint8_t* out_palette_rgb_host, int32_t* entries_host, int32_t w_expected,
+                         int32_t h_expected);
+/* file i -> outs_index_host[i], palettes_rgb_host + i * 768, entries_host[i]; per-file codes in rcs_host as rsb_png_read_rgb_batch */
+int rsb_png_read_indexed_batch(const char* const* paths, int32_t n, uint8_t* const* outs_index_host, uint8_t* palettes_rgb_host,
+                               int32_t* entries_host, int32_t w_expected, int32_t h_expected, int32_t threads, int32_t* rcs_host);
+/* `combined.save(path, optimize=True)` of `rs compare` (compare.py:66-67): 8-bit RGB PNG (colour type 2) of pixels_host uint8
+ * [h][w][3], with rsb_png_encode_p8's level and Z_RLE policy; same pixels as PIL's file, different compressed bytes. */
+int64_t rsb_png_encode_rgb8(const uint8_t* pixels_host, int32_t w, int32_t h, int32_t level, uint8_t* out_host, int64_t capacity);
+/* image i is pixels_host + i * image_stride; make_dirs != 0 creates the parent directories (z/x/) */
+int rsb_png_write_rgb8_batch(const char* const* paths, int32_t n, const uint8_t* pixels_host, int64_t image_stride, int32_t w, int32_t h,
+                             int32_t level, int32_t threads, int32_t make_dirs);
 
 /* ---------------------------------------------------------------------------------------------
  * Losses and metrics on fp32 NCHW logits + int64 targets [N][H][W].

@@ -99,6 +99,7 @@ RSB_PBF_SEG_FIELDS = 16
  RSB_PBF_SEG_LON_OFF, RSB_PBF_SEG_LON_LEN, RSB_PBF_SEG_GRANULARITY, RSB_PBF_SEG_LAT_OFFSET, RSB_PBF_SEG_LON_OFFSET, RSB_PBF_SEG_HOST_FIRST,
  RSB_PBF_SEG_OUT_FIRST) = range(14)
 RSB_EXTRACT_WARP_RING = 256
+RSB_COMPARE_MAX_PLANES = 32
 
 
 class MorphOp(ctypes.Structure):
@@ -226,6 +227,13 @@ SIGNATURES = {
     "rsb_png_write_p8": (ctypes.c_int, [ctypes.c_char_p, _vp, _i32, _i32, _vp, _i32, _i32]),
     "rsb_png_read_rgb_batch": (ctypes.c_int, [_vp, _i32, _vp, _i32, _i32, _i32, _vp]),
     "rsb_png_write_p8_batch": (ctypes.c_int, [_vp, _i32, _vp, _i64, _i32, _i32, _vp, _i32, _i32, _i32, _i32]),
+    "rsb_png_decode_indexed": (ctypes.c_int, [_vp, _i64, _vp, _vp, _vp, _i32, _i32]),
+    "rsb_png_read_indexed": (ctypes.c_int, [ctypes.c_char_p, _vp, _vp, _vp, _i32, _i32]),
+    "rsb_png_read_indexed_batch": (ctypes.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "rsb_png_encode_rgb8": (_i64, [_vp, _i32, _i32, _i32, _vp, _i64]),
+    "rsb_png_write_rgb8_batch": (ctypes.c_int, [_vp, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _i32]),
+    "rsb_compare_count": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp]),
+    "rsb_compare_compose": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i64, _vp, _i64, _vp]),
     "rsb_softmax_nchw": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_cross_entropy": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_focal": (ctypes.c_int, [_vp, _vp, _vp, _f32, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),

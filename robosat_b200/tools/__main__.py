@@ -1,9 +1,9 @@
-"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe,merge,extract} ...` -- the `rs`
-sub-commands on the hot path (dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
+"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe,merge,extract,compare} ...` --
+the `rs` sub-commands on the hot path (dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
 
 import argparse
 
-from robosat_b200.tools import cover, dedupe, extract, features, masks, merge, predict, rasterize, serve, train, weights
+from robosat_b200.tools import compare, cover, dedupe, extract, features, masks, merge, predict, rasterize, serve, train, weights
 
 
 def add_parsers():
@@ -20,6 +20,7 @@ def add_parsers():
     dedupe.add_parser(subparser)
     merge.add_parser(subparser)
     extract.add_parser(subparser)
+    compare.add_parser(subparser)
     subparser.required = True
     return parser.parse_args()
 
