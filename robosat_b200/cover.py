@@ -19,7 +19,7 @@ import math
 import numpy as np
 
 from robosat_b200 import _lib
-from robosat_b200.rasterize import INVALID_ERRORS, W_INVALID, PolygonSet, polygon_to_mercator
+from robosat_b200.rasterize import INVALID_ERRORS, W_INVALID, PolygonSet, fill_bands, polygon_to_mercator
 
 R = 6378137.0
 MAX_LAT = 85.0511287798066  # supermercado clamps the latitude extrema to Web Mercator's square
@@ -27,7 +27,6 @@ SHRINK = 1e-10  # supermercado shrinks the lon/lat extrema by this much on each 
 DEFAULT_BUDGET = 1 << 30
 # device bytes per grid cell of a batch, beyond its bitmap: an int64 key per cell at most, plus the sort's two padded key buffers
 KEY_BYTES_PER_CELL = 25
-FILL_WORDS = 12288  # bitmap words of a fill CTA's band in shared memory (48 KB) unless a single row needs more
 W_GEOMETRY = "Warning: feature {} is a {}, not a Polygon or MultiPolygon, skipping"
 
 
@@ -202,13 +201,7 @@ def _batch_args(fs, grids, jobs):
     np.cumsum(rows * words, out=bitmap_offsets[1:])
     if bitmap_offsets[-1] == 0:
         return None
-    max_words = int(words[rows > 0].max())
-    band_rows = max(1, min(128, FILL_WORDS // max_words))
-    nb = (rows + band_rows - 1) // band_rows
-    band_feature = np.repeat(np.arange(F), nb)
-    band_index = np.arange(len(band_feature)) - np.repeat(np.cumsum(nb) - nb, nb)
-    band_start = band_index * band_rows
-    bands = np.stack([band_feature, band_start, np.minimum(band_rows, rows[band_feature] - band_start)], axis=1).astype(np.int32)
+    bands, band_rows, max_words = fill_bands(rows, words)
     if len(bands) > 0x7fffffff:
         raise _lib.RsbError("%d fill bands in one batch" % len(bands))
 

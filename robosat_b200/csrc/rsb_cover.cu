@@ -9,9 +9,9 @@
 // The walk is a sequential float64 recurrence along one edge, so it cannot be split: one thread walks one edge from its own
 // clipped start, exactly as the restatement does (tests/cover_reference.py), and sets bits with atomicOr in the global bitmap.
 // A long edge is therefore walked once, not once per band of the fill; edges, not bands, carry the walk's parallelism. The fill
-// then runs one CTA per (feature, band of rows) with the toggle + prefix-XOR scheme of rsb_raster.cu, generalised to W != H and
-// to rows of up to RSB_COVER_MAX_WIDTH columns, and ORs its rows into the same bitmap (the bands of a launch are disjoint, and the
-// walk kernel has finished, so plain stores suffice). Bits are OR-ed, so the bitmap does not depend on the order of anything.
+// then runs one CTA per (feature, band of rows) with fill_band (rsb_geom.cuh) on rows of up to RSB_COVER_MAX_WIDTH columns, and
+// ORs its rows into the same bitmap (the bands of a launch are disjoint, and the walk kernel has finished, so plain stores
+// suffice). Bits are OR-ed, so the bitmap does not depend on the order of anything.
 //
 // Keys are (x << zoom) | y, so ascending keys are tiles in (x, y) order. rsb_cover_emit_keys writes one key per set bit in an
 // unspecified order; rsb_sort_unique_u64 sorts them with a stable LSD radix sort of ceil(key_bits / 8) 8-bit passes (the
@@ -26,6 +26,7 @@
 #include <algorithm>
 
 #include "../../include/rsb200.h"
+#include "rsb_geom.cuh"
 #include "rsb_host.h"
 
 using namespace rsb;
@@ -49,21 +50,6 @@ struct CoverGrid {
 __device__ __forceinline__ CoverGrid load_grid(const int64_t* __restrict__ g, int f) {
     const int64_t* p = g + 6 * static_cast<int64_t>(f);
     return CoverGrid{p[0], p[1], p[2], p[3], p[4], p[5]};
-}
-
-__device__ __forceinline__ double2 to_pixels(const double* __restrict__ v, int64_t i, double c0, double c1, double r0, double r1) {
-    const double2 m = reinterpret_cast<const double2*>(v)[i];
-    return make_double2(__dadd_rn(c0, __dmul_rn(m.x, c1)), __dadd_rn(r0, __dmul_rn(m.y, r1)));
-}
-
-// first index in [lo, hi) with a[index] > v (hi when none)
-__device__ __forceinline__ int64_t upper_bound(const int64_t* __restrict__ a, int64_t lo, int64_t hi, int64_t v) {
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (a[mid] <= v) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
 }
 
 __device__ __forceinline__ void burn_cell(uint32_t* __restrict__ bm, const CoverGrid& g, int64_t words, int64_t ix, int64_t iy) {
@@ -189,93 +175,16 @@ __global__ void __launch_bounds__(FILL_THREADS) cover_fill_kernel(const double* 
                                                                   const int64_t* __restrict__ bitmap_offsets, const int32_t* __restrict__ bands,
                                                                   uint32_t* __restrict__ bitmap) {
     extern __shared__ __align__(16) uint32_t tog[];
-    __shared__ int s_rmin, s_rmax;
     const int f = bands[3 * blockIdx.x], band_row = bands[3 * blockIdx.x + 1], rows = bands[3 * blockIdx.x + 2];
     const CoverGrid g = load_grid(grids, f);
     const int words = static_cast<int>((g.W + 31) >> 5);
-    const int64_t y0 = g.row_lo + band_row;  // first grid row of the band
     uint32_t* out = bitmap + bitmap_offsets[f] + static_cast<int64_t>(band_row) * words;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
-    for (int i = tid; i < rows * words; i += blockDim.x) tog[i] = 0u;
-    if (tid == 0) {
-        s_rmin = INT32_MAX;
-        s_rmax = -1;
-    }
-    const double c0 = transforms[4 * f + 0], c1 = transforms[4 * f + 1], r0 = transforms[4 * f + 2], r1 = transforms[4 * f + 3];
-    const double band_lo = static_cast<double>(y0), band_hi = static_cast<double>(y0 + rows), Wd = static_cast<double>(g.W);
-    const uint32_t tail = (g.W & 31) ? (1u << (g.W & 31)) - 1u : FULL;  // valid bits of a row's last word
-    __syncthreads();
-
-    for (int p = feature_polys[f]; p < feature_polys[f + 1]; ++p) {
-        int rlo = INT32_MAX, rhi = -1;
-        for (int ring = poly_rings[p]; ring < poly_rings[p + 1]; ++ring) {
-            const int64_t v0 = ring_offsets[ring], v1 = ring_offsets[ring + 1];
-            for (int64_t i = v0 + tid; i < v1; i += blockDim.x) {
-                double2 a = to_pixels(vertices, i, c0, c1, r0, r1);
-                double2 b = to_pixels(vertices, i + 1 < v1 ? i + 1 : v0, c0, c1, r0, r1);
-                if (a.y > b.y) {
-                    const double2 t = a;
-                    a = b;
-                    b = t;
-                }
-                // rows with y1 <= r + 0.5 < y2 inside the band; start one row early and test exactly
-                if (!(a.y < band_hi && b.y > band_lo && a.y < b.y)) continue;
-                const double start = fmax(floor(a.y - 0.5), band_lo);
-                const double dx = __dsub_rn(b.x, a.x), dy = __dsub_rn(b.y, a.y);
-                for (int r = static_cast<int>(start - band_lo); r < rows; ++r) {
-                    const double yc = static_cast<double>(y0 + r) + 0.5;
-                    if (!(yc < b.y)) break;
-                    if (!(a.y <= yc)) continue;
-                    const double x = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(yc, a.y), dx), dy), a.x);
-                    const double c = fmin(fmax(floor(__dadd_rn(x, 0.5)), 0.0), Wd);
-                    const int64_t col = static_cast<int64_t>(c);
-                    if (col < g.W) atomicXor(&tog[r * words + static_cast<int>(col >> 5)], 1u << (col & 31));
-                    rlo = min(rlo, r);
-                    rhi = max(rhi, r);
-                }
-            }
-        }
-        const int hit = rhi >= 0;
-        if (hit) {
-            atomicMin(&s_rmin, rlo);
-            atomicMax(&s_rmax, rhi);
-        }
-        if (!__syncthreads_or(hit)) continue;
-        const int lo = s_rmin, hi = s_rmax;
-        __syncthreads();
-        if (tid == 0) {
-            s_rmin = INT32_MAX;
-            s_rmax = -1;
-        }
-        for (int r = lo + warp; r <= hi; r += nwarps) {
-            uint32_t carry = 0;  // parity of all toggles left of this chunk
-            for (int c0w = 0; c0w < words; c0w += 32) {
-                const int w = c0w + lane;
-                uint32_t t = 0;
-                if (w < words) {
-                    t = tog[r * words + w];
-                    tog[r * words + w] = 0u;
-                }
-                t ^= t << 1;
-                t ^= t << 2;
-                t ^= t << 4;
-                t ^= t << 8;
-                t ^= t << 16;
-                uint32_t par = t >> 31;
-                for (int o = 1; o < 32; o <<= 1) {
-                    const uint32_t u = __shfl_up_sync(FULL, par, o);
-                    if (lane >= o) par ^= u;
-                }
-                const uint32_t excl = (par ^ (t >> 31)) ^ carry;
-                if (w < words) {
-                    const uint32_t bits = (excl ? ~t : t) & (w == words - 1 ? tail : FULL);
-                    if (bits) out[static_cast<int64_t>(r) * words + w] |= bits;
-                }
-                carry = __shfl_sync(FULL, par, 31) ^ carry;
-            }
-        }
-        __syncthreads();
-    }
+    for (int i = threadIdx.x; i < rows * words; i += blockDim.x) tog[i] = 0u;
+    fill_band(
+        vertices, ring_offsets, poly_rings, feature_polys[f], feature_polys[f + 1], [](int k) { return k; }, transforms[4 * f + 0], transforms[4 * f + 1],
+        transforms[4 * f + 2], transforms[4 * f + 3], g.W, g.row_lo + band_row, rows, tog, [&](int r, int w, uint32_t bits) {
+            if (bits) out[static_cast<int64_t>(r) * words + w] |= bits;
+        });
 }
 
 // popcount of the batch's bitmap into status[0]; with keys, also one key per set bit at slots taken from status[2]

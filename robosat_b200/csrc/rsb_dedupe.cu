@@ -32,6 +32,7 @@
 #include <algorithm>
 
 #include "../../include/rsb200.h"
+#include "rsb_geom.cuh"
 #include "rsb_host.h"
 
 using namespace rsb;
@@ -348,16 +349,6 @@ __device__ void fractions(const Edge& e, const Context& cx, int k, bool near_p, 
         pr.tm = __dmul_rn(0.5, __dadd_rn(t0, t1));
         pr.m = make_double2(__dadd_rn(e.a.x, __dmul_rn(pr.tm, e.d.x)), __dadd_rn(e.a.y, __dmul_rn(pr.tm, e.d.y)));
     }
-}
-
-// first index in [lo, hi) with a[index] > v
-__device__ __forceinline__ int64_t upper_bound(const int64_t* __restrict__ a, int64_t lo, int64_t hi, int64_t v) {
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (a[mid] <= v) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
 }
 
 __global__ void __launch_bounds__(AREA_THREADS) dedupe_terms_kernel(Shapes P, Shapes Q, const int32_t* __restrict__ pred, const double* __restrict__ origins,

@@ -16,7 +16,7 @@
 // smallest index of i's component on every run.
 //
 // rsb_merge_fill: one CTA per (component, band of rows) sets the cells whose centres the component's polygons cover, with the
-// toggle + prefix-XOR scanline fill of rsb_cover.cu (even-odd per polygon, union across polygons) on bit-packed rows.
+// scanline fill of rsb_geom.cuh (even-odd per polygon, union across polygons) on bit-packed rows.
 //
 // rsb_merge_close: one CTA per (component, tile of 32 rows x 32 words) computes erode(dilate(fill)) with the digital disk
 // {(i, j): i^2 + j^2 <= K^2}: the tile's rows plus 2K halo rows and 2 halo words on each side are staged in shared memory,
@@ -30,6 +30,7 @@
 #include <algorithm>
 
 #include "../../include/rsb200.h"
+#include "rsb_geom.cuh"
 #include "rsb_host.h"
 
 using namespace rsb;
@@ -136,11 +137,6 @@ __global__ void __launch_bounds__(UF_THREADS) uf_jump_kernel(int32_t* parent, in
 
 // ---- fill ----
 
-__device__ __forceinline__ double2 to_cells(const double* __restrict__ v, int64_t i, double c0, double c1, double r0, double r1) {
-    const double2 m = reinterpret_cast<const double2*>(v)[i];
-    return make_double2(__dadd_rn(c0, __dmul_rn(m.x, c1)), __dadd_rn(r0, __dmul_rn(m.y, r1)));
-}
-
 // one CTA per band: bands[3 * b] = (component, first row, rows); grids[2 * c] = (W, H)
 __global__ void __launch_bounds__(FILL_THREADS, 1) merge_fill_kernel(const double* __restrict__ vertices, const int64_t* __restrict__ ring_offsets,
                                                                   const int32_t* __restrict__ poly_rings, const int32_t* __restrict__ comp_poly_offsets,
@@ -148,92 +144,17 @@ __global__ void __launch_bounds__(FILL_THREADS, 1) merge_fill_kernel(const doubl
                                                                   const int64_t* __restrict__ grids, const int64_t* __restrict__ bitmap_offsets,
                                                                   const int32_t* __restrict__ bands, uint32_t* __restrict__ bitmap) {
     extern __shared__ __align__(16) uint32_t tog[];
-    __shared__ int s_rmin, s_rmax;
     const int c = bands[3 * blockIdx.x], band_row = bands[3 * blockIdx.x + 1], rows = bands[3 * blockIdx.x + 2];
     const int64_t W = grids[2 * c];
     const int words = static_cast<int>((W + 31) >> 5);
     uint32_t* out = bitmap + bitmap_offsets[c] + static_cast<int64_t>(band_row) * words;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
-    for (int i = tid; i < rows * words; i += blockDim.x) tog[i] = 0u;
-    if (tid == 0) {
-        s_rmin = INT32_MAX;
-        s_rmax = -1;
-    }
-    const double c0 = transforms[4 * c + 0], c1 = transforms[4 * c + 1], r0 = transforms[4 * c + 2], r1 = transforms[4 * c + 3];
-    const double band_lo = static_cast<double>(band_row), band_hi = static_cast<double>(band_row + rows), Wd = static_cast<double>(W);
-    const uint32_t tail = (W & 31) ? (1u << (W & 31)) - 1u : FULL;
-    __syncthreads();
-
-    for (int k = comp_poly_offsets[c]; k < comp_poly_offsets[c + 1]; ++k) {
-        const int p = comp_polys[k];
-        int rlo = INT32_MAX, rhi = -1;
-        for (int ring = poly_rings[p]; ring < poly_rings[p + 1]; ++ring) {
-            const int64_t v0 = ring_offsets[ring], v1 = ring_offsets[ring + 1];
-            for (int64_t i = v0 + tid; i < v1; i += blockDim.x) {
-                double2 a = to_cells(vertices, i, c0, c1, r0, r1);
-                double2 b = to_cells(vertices, i + 1 < v1 ? i + 1 : v0, c0, c1, r0, r1);
-                if (a.y > b.y) {
-                    const double2 t = a;
-                    a = b;
-                    b = t;
-                }
-                if (!(a.y < band_hi && b.y > band_lo && a.y < b.y)) continue;
-                const double start = fmax(floor(a.y - 0.5), band_lo);
-                const double dx = __dsub_rn(b.x, a.x), dy = __dsub_rn(b.y, a.y);
-                for (int r = static_cast<int>(start - band_lo); r < rows; ++r) {
-                    const double yc = static_cast<double>(band_row + r) + 0.5;
-                    if (!(yc < b.y)) break;
-                    if (!(a.y <= yc)) continue;
-                    const double x = __dadd_rn(__ddiv_rn(__dmul_rn(__dsub_rn(yc, a.y), dx), dy), a.x);
-                    const double cc = fmin(fmax(floor(__dadd_rn(x, 0.5)), 0.0), Wd);
-                    const int64_t col = static_cast<int64_t>(cc);
-                    if (col < W) atomicXor(&tog[r * words + static_cast<int>(col >> 5)], 1u << (col & 31));
-                    rlo = min(rlo, r);
-                    rhi = max(rhi, r);
-                }
-            }
-        }
-        const int hit = rhi >= 0;
-        if (hit) {
-            atomicMin(&s_rmin, rlo);
-            atomicMax(&s_rmax, rhi);
-        }
-        if (!__syncthreads_or(hit)) continue;
-        const int lo = s_rmin, hi = s_rmax;
-        __syncthreads();
-        if (tid == 0) {
-            s_rmin = INT32_MAX;
-            s_rmax = -1;
-        }
-        for (int r = lo + warp; r <= hi; r += nwarps) {
-            uint32_t carry = 0;  // parity of all toggles left of this chunk
-            for (int cw = 0; cw < words; cw += 32) {
-                const int w = cw + lane;
-                uint32_t t = 0;
-                if (w < words) {
-                    t = tog[r * words + w];
-                    tog[r * words + w] = 0u;
-                }
-                t ^= t << 1;
-                t ^= t << 2;
-                t ^= t << 4;
-                t ^= t << 8;
-                t ^= t << 16;
-                uint32_t par = t >> 31;
-                for (int o = 1; o < 32; o <<= 1) {
-                    const uint32_t u = __shfl_up_sync(FULL, par, o);
-                    if (lane >= o) par ^= u;
-                }
-                const uint32_t excl = (par ^ (t >> 31)) ^ carry;
-                if (w < words) {
-                    const uint32_t bits = (excl ? ~t : t) & (w == words - 1 ? tail : FULL);
-                    if (bits) out[static_cast<int64_t>(r) * words + w] |= bits;
-                }
-                carry = __shfl_sync(FULL, par, 31) ^ carry;
-            }
-        }
-        __syncthreads();
-    }
+    for (int i = threadIdx.x; i < rows * words; i += blockDim.x) tog[i] = 0u;
+    fill_band(
+        vertices, ring_offsets, poly_rings, comp_poly_offsets[c], comp_poly_offsets[c + 1], [&](int k) { return comp_polys[k]; }, transforms[4 * c + 0],
+        transforms[4 * c + 1], transforms[4 * c + 2], transforms[4 * c + 3], W, band_row, rows, tog,
+        [&](int r, int w, uint32_t bits) {
+            if (bits) out[static_cast<int64_t>(r) * words + w] |= bits;
+        });
 }
 
 // ---- closing ----

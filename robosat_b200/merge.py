@@ -31,7 +31,8 @@ from robosat_b200 import _lib
 from robosat_b200 import dedupe as DD
 from robosat_b200 import features as FT
 from robosat_b200.cover import _alloc
-from robosat_b200.rasterize import INVALID_ERRORS, W_INVALID
+# FILL_WORDS, the band budget of rsb_merge_fill, is defined once in rasterize and stays readable as merge.FILL_WORDS
+from robosat_b200.rasterize import FILL_WORDS, INVALID_ERRORS, W_INVALID, fill_bands  # noqa: F401
 
 A = 6378137.0  # WGS84
 FLATTENING = 1 / 298.257223563
@@ -40,7 +41,6 @@ PHI2_ITER, PHI2_TOL = 15, 1e-10  # PROJ's pj_phi2
 CELLS_PER_THRESHOLD = 4  # K: cells per threshold distance, and the radius of the closing's disk in cells
 MARGIN = CELLS_PER_THRESHOLD + 2  # cells around a component's box, so that the dilation never reaches the grid edge
 DEFAULT_BUDGET = 1 << 30
-FILL_WORDS = 12288  # bitmap words of a fill CTA's band in shared memory (48 KB) unless a single row needs more
 TILE_ROWS, TILE_WORDS = 32, 32  # a closing CTA's tile
 COMPONENT_BYTES = 64  # device bytes per component beyond its two bitmaps: transforms, grid, offsets, bands, tiles (upper bound)
 W_GEOMETRY = "Warning: {} features are not a Polygon or MultiPolygon, skipping them"
@@ -263,12 +263,7 @@ def close_device(shapes, comps, device="cuda", stats=None, keep_fill=False):
     polys = [np.concatenate([np.arange(fp[f], fp[f + 1]) for f in c.members]) for c in comps]
     poly_offsets = np.zeros(C + 1, np.int64)
     np.cumsum([len(x) for x in polys], out=poly_offsets[1:])
-    max_words = int(words.max())
-    band_rows = max(1, min(128, FILL_WORDS // max_words))
-    nb = (H + band_rows - 1) // band_rows
-    bc = np.repeat(np.arange(C), nb)
-    b0 = (np.arange(len(bc)) - np.repeat(np.cumsum(nb) - nb, nb)) * band_rows
-    bands = np.stack([bc, b0, np.minimum(band_rows, H[bc] - b0)], axis=1)
+    bands, band_rows, max_words = fill_bands(H, words)
     tr, tw = (H + TILE_ROWS - 1) // TILE_ROWS, (words + TILE_WORDS - 1) // TILE_WORDS
     nt = tr * tw
     tc = np.repeat(np.arange(C), nt)

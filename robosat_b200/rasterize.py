@@ -16,6 +16,7 @@ from robosat_b200 import _lib
 
 R = 6378137.0  # EPSG:3857 sphere radius
 CE = 2 * math.pi * R
+FILL_WORDS = 12288  # bitmap words of a fill CTA's band in shared memory (48 KB) unless a single row needs more
 
 
 def project(lonlat):
@@ -104,6 +105,21 @@ class PolygonSet:
         self.d_vertices = torch.from_numpy(self.vertices if len(self.vertices) else np.zeros((1, 2))).to(device)
         self.d_ring_offsets = torch.from_numpy(self.ring_offsets).to(device)
         self.d_poly_rings = torch.from_numpy(self.poly_rings).to(device)
+
+
+def fill_bands(rows, words):
+    """The bands of the grid fill of `rs cover` and `rs merge`, one CTA each, for items of `rows` rows of `words` bitmap words
+    (at least one item has rows) -> (bands int32 [n, 3] = (item, first row, rows), band_rows, max_words). Every row of every
+    item is in one band; a band has at most band_rows = min(128, FILL_WORDS // max_words) rows (at least one), max_words being
+    the widest item with rows."""
+    rows = np.asarray(rows, np.int64)
+    max_words = int(np.asarray(words, np.int64)[rows > 0].max())
+    band_rows = max(1, min(128, FILL_WORDS // max_words))
+    nb = (rows + band_rows - 1) // band_rows
+    item = np.repeat(np.arange(len(rows)), nb)
+    start = (np.arange(len(item)) - np.repeat(np.cumsum(nb) - nb, nb)) * band_rows
+    bands = np.stack([item, start, np.minimum(band_rows, rows[item] - start)], axis=1).astype(np.int32)
+    return bands, band_rows, max_words
 
 
 def bin_polygons(tiles, bboxes):

@@ -1,6 +1,6 @@
 """`rs rasterize` on the CPU: the numpy restatement of GDAL's fill against the reference's golden parking masks, the reference's own
-assertions, projection and tile bounds, binning against a brute-force cover, feature filtering, the command line and the C entry
-point's validation."""
+assertions, projection and tile bounds, binning against a brute-force cover, the fill bands of `rs cover` and `rs merge`, feature
+filtering, the command line and the C entry point's validation."""
 
 import argparse
 import ctypes
@@ -117,6 +117,25 @@ def test_polygon_set_packing():
     assert len(ps) == 3
     assert ps.ring_offsets.tolist() == [0, 4, 8, 12] and ps.poly_rings.tolist() == [0, 2, 2, 3]
     assert ps.bboxes[0].tolist() == [0, 0, 1, 1] and np.isnan(ps.bboxes[1]).all() and ps.bboxes[2].tolist() == [4, -1, 6, 3]
+
+
+@pytest.mark.parametrize("items", [
+    [(4, 1), (0, 0), (100, 1), (300, 2)],  # narrow grids: bands of 128 rows, an empty window between them
+    [(5000, 200), (1, 3)],  # 61 rows of 200 words fit in FILL_WORDS
+    [(3, 20000), (7, 5)],  # one row wider than FILL_WORDS: bands of one row
+    [(0, 50000), (10, 100)],  # a wide item without rows does not set the width
+])
+def test_fill_bands_cover_every_row_once(items):
+    rows, words = np.array(items, np.int64).T
+    bands, band_rows, max_words = RZ.fill_bands(rows, words)
+    assert bands.dtype == np.int32 and bands.shape == (len(bands), 3)
+    assert max_words == words[rows > 0].max()
+    assert 1 <= band_rows <= 128 and (band_rows * max_words <= RZ.FILL_WORDS or max_words > RZ.FILL_WORDS)
+    assert (bands[:, 2] >= 1).all() and (bands[:, 2] <= band_rows).all()
+    assert bands[:, 2].sum() == rows.sum()
+    for i, n in enumerate(rows):
+        mine = bands[bands[:, 0] == i]
+        assert sorted(r for _, start, count in mine for r in range(start, start + count)) == list(range(n))
 
 
 def _poly(lonlat):
