@@ -595,44 +595,27 @@ int rsb_adam_step_guarded(float* param, const float* grad, float* exp_avg, float
  * Training path (robosat/tools/train.py:163-201: net.train() forward, loss.backward()). Activations and activation
  * gradients are NHWC fp16 [M = N*H*W][C]; gradients carry the caller's loss scale; parameter gradients are fp32, unscaled.
  */
-/* train-mode BatchNorm2d (torchvision resnet50 inside unet.py:122-130): batch sums -> statistics / running-stat update -> apply.
- * sums: 20*C doubles of scratch (8 replicated accumulator slots, arrival counter, backward coefficients). finalize writes mean, invstd, scale = gamma*invstd, shift = beta - mean*scale and updates
- * running_mean / running_var (unbiased, momentum) / num_batches_tracked when those pointers are non-NULL. */
-int rsb_bn_stats(const void* z, double* sums, int64_t M, int32_t C, void* stream);
-int rsb_bn_finalize(const double* sums, const float* gamma, const float* beta, float* running_mean, float* running_var,
-                    int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int32_t C, int64_t M, float eps,
-                    float momentum, void* stream);
-/* rsb_bn_stats + rsb_bn_finalize in one launch (the last block of the reduction does the per-channel epilogue) */
-int rsb_bn_stats_finalize(const void* z, double* sums, const float* gamma, const float* beta, float* running_mean, float* running_var,
-                          int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int64_t M, int32_t C, float eps,
-                          float momentum, void* stream);
-/* "_chained" variants (what the training plan uses): the same arithmetic, but (a) launched with programmatic stream serialization
- * so a chain of small kernels does not pay a full launch gap per link, and (b) without the per-call memset: `sums` must be
- * zero-initialised ONCE by the caller and is left zeroed by the reduction's last block. */
-int rsb_bn_stats_finalize_chained(const void* z, double* sums, const float* gamma, const float* beta, float* running_mean, float* running_var,
-                                  int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int64_t M, int32_t C, float eps,
-                                  float momentum, void* stream);
-/* Same statistics / finalize from the per-quarter-tile partial sums a convolution wrote through rsb_conv_desc.stats
- * (partials: fp32 [rows][2][C], rows = spatial tiles * 4) instead of re-reading z: 1/8 of the bytes. `chained` as above
- * (1: no memset, programmatic stream serialization; sums must be zero on entry and is left zeroed). */
+/* train-mode BatchNorm2d (torchvision resnet50 inside unet.py:122-130): batch statistics -> apply -> backward, each launched with
+ * programmatic stream serialization so that a chain of small kernels does not pay a full launch gap per link.
+ * sums: 20*C doubles of scratch (8 replicated accumulator slots, arrival counter, backward coefficients), zero-initialised ONCE by
+ * the caller: the last block of each reduction leaves it zeroed again, and no call clears it with a memset. The "_chained" suffix
+ * marks these semantics. */
+/* batch statistics from the per-quarter-tile partial sums a convolution wrote through rsb_conv_desc.stats (partials: fp32
+ * [rows][2][C], rows = spatial tiles * 4; 1/8 of the bytes of z): mean, invstd, scale = gamma*invstd, shift = beta - mean*scale,
+ * and running_mean / running_var (unbiased, momentum) / num_batches_tracked updated when those pointers are non-NULL. */
 int rsb_bn_partials_finalize(const float* partials, int64_t rows, double* sums, const float* gamma, const float* beta, float* running_mean,
                              float* running_var, int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int64_t M,
-                             int32_t C, float eps, float momentum, int32_t chained, void* stream);
+                             int32_t C, float eps, float momentum, void* stream);
+/* y = relu?(z*scale + shift (+ residual)) */
 int rsb_bn_apply_chained(const void* z, const float* scale, const float* shift, const void* residual, void* y, int64_t M, int32_t C,
                          int32_t relu, void* stream);
+/* autograd of relu(bn(z) (+ identity)): g = dy * (y > 0) (y NULL: no mask); dz = gamma*invstd*(g - mean(g) - zhat*mean(g*zhat));
+ * g_out (optional) receives g = the gradient of the identity branch; dgamma/dbeta fp32 multiplied by inv_loss_scale.
+ * mask_scale / mask_shift (with y NULL): the output was the plain y = half(relu(z*scale + shift)) of rsb_bn_apply_chained, so its
+ * ReLU mask is re-derived from z (bit-identical: half(o) > 0 <=> o > 2^-25) and y is not read at all. */
 int rsb_bn_backward_chained(const void* dy, const void* y, const void* z, const float* mean, const float* invstd, const float* gamma,
                             const float* mask_scale, const float* mask_shift, double* sums, void* dz, void* g_out, float* dgamma, float* dbeta,
                             float inv_loss_scale, int64_t M, int32_t C, void* stream);
-/* y = relu?(z*scale + shift (+ residual)) */
-int rsb_bn_apply(const void* z, const float* scale, const float* shift, const void* residual, void* y, int64_t M, int32_t C,
-                 int32_t relu, void* stream);
-/* autograd of relu(bn(z) (+ identity)): g = dy * (y > 0) (y NULL: no mask); dz = gamma*invstd*(g - mean(g) - zhat*mean(g*zhat));
- * g_out (optional) receives g = the gradient of the identity branch; dgamma/dbeta fp32 multiplied by inv_loss_scale.
- * mask_scale / mask_shift (with y NULL): the output was the plain y = half(relu(z*scale + shift)) of rsb_bn_apply, so its ReLU mask
- * is re-derived from z (bit-identical: half(o) > 0 <=> o > 2^-25) and y is not read at all. */
-int rsb_bn_backward(const void* dy, const void* y, const void* z, const float* mean, const float* invstd, const float* gamma,
-                    const float* mask_scale, const float* mask_shift, double* sums, void* dz, void* g_out, float* dgamma, float* dbeta,
-                    float inv_loss_scale, int64_t M, int32_t C, void* stream);
 /* out = (a (+ b)) * (y > 0): ReLU backward with optional gradient fan-in (skip connections); y NULL: plain sum */
 int rsb_relu_backward(const void* a, const void* b, const void* y, void* out, int64_t n, void* stream);
 /* autograd of max_pool2d (unet.py:125, :132) on NHWC fp16: first maximum of every window receives its gradient.
@@ -654,24 +637,22 @@ int rsb_pack_weights(const float* src, const int32_t* map4, void* dst, int64_t n
 /* the same with ONE source index per packed element (map1: int32 [n], -1 = zero; n a multiple of 8, map1 and dst 16-byte
  * aligned): a quarter of the map bytes; used for every layout but the pre-summed nearest-x2 taps */
 int rsb_pack_weights1(const float* src, const int32_t* map1, void* dst, int64_t n, void* stream);
-/* packed fp32 gradient -> OIHW fp32 gradient: grad[map4[4i+j]] += packed_grad[i] * mul (the transpose of rsb_pack_weights) */
-int rsb_unpack_grads(const float* packed_grad, const int32_t* map4, float* grad, int64_t n, float mul, void* stream);
-
-/* the same reduction without atomics (deterministic): element i of the compact list writes grad[dst_idx[i]] = mul * (sum of the
- * packed gradient elements inv4[4i..4i+3], entries < 0 skipped, added in index order); inv4 is the inverse of map4 */
+/* packed fp32 gradient -> OIHW fp32 gradient, the transpose of rsb_pack_weights, without atomics (deterministic): element i of the
+ * compact list writes grad[dst_idx[i]] = mul * (sum of the packed gradient elements inv4[4i..4i+3], entries < 0 skipped, added in
+ * index order); inv4 is the inverse of the pack map4 (robosat_b200.train_engine.invert_unpack_map) */
 int rsb_unpack_grads_gather(const float* packed_grad, const int32_t* dst_idx, const int32_t* inv4, float* grad, int64_t n, float mul,
                             void* stream);
 
 /* Weight gradient of the convolution described by `fwd` (same sources / segments / phases / tile space), on tensor cores:
  *   dw_packed[phase*Cout + co][k] = sum_pixels dy_phase[pixel][co] * x_segment(k)[pixel + (dh,dw)][k % 64-block]   (fp32)
- * i.e. the gradient in the forward kernel's packed weight layout (rsb_unpack_grads folds it back to OIHW).
+ * i.e. the gradient in the forward kernel's packed weight layout (rsb_unpack_grads_gather folds it back to OIHW).
  * dy is addressed like fwd->out (same pitches / phase strides). Replaces autograd's conv weight gradients (train.py:186). */
 typedef struct rsb_wgrad_plan rsb_wgrad_plan;
 int rsb_wgrad_plan_create(const rsb_conv_desc* fwd, const void* dy, float* dw_packed, rsb_wgrad_plan** out_plan);
-/* Deterministic split-K: bytes of scratch the plan needs (0 when it has a single pixel slice), and the call that hands it over.
- * With a scratch every slice stores its partial gradient and a second kernel adds the slices in index order (bit-identical from
- * run to run); without one the slices add into dw_packed with fp32 atomics. The scratch is private to a launch and may be shared
- * by all plans that run on one stream. */
+/* Split-K: bytes of scratch the plan needs (0 when it has a single pixel slice), and the call that hands it over. Every slice
+ * stores its partial gradient there and a second kernel adds the slices in index order (bit-identical from run to run). A plan
+ * that needs a scratch must get one before rsb_wgrad_run, which otherwise returns RSB_E_INVALID and launches nothing. The scratch
+ * is private to a launch and may be shared by all plans that run on one stream. */
 int64_t rsb_wgrad_plan_scratch_bytes(const rsb_wgrad_plan* plan);
 int rsb_wgrad_plan_set_scratch(rsb_wgrad_plan* plan, float* scratch, int64_t scratch_bytes);
 void rsb_wgrad_plan_destroy(rsb_wgrad_plan* plan);

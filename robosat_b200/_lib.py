@@ -244,15 +244,9 @@ SIGNATURES = {
     "rsb_metrics_count": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_adam_step": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _i32, _vp]),
     "rsb_adam_step_guarded": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _i32, _vp, _vp]),
-    "rsb_bn_stats": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp]),
-    "rsb_bn_stats_finalize": (ctypes.c_int, [_vp] * 11 + [_i64, _i32, _f32, _f32, _vp]),
-    "rsb_bn_stats_finalize_chained": (ctypes.c_int, [_vp] * 11 + [_i64, _i32, _f32, _f32, _vp]),
     "rsb_bn_apply_chained": (ctypes.c_int, [_vp] * 5 + [_i64, _i32, _i32, _vp]),
     "rsb_bn_backward_chained": (ctypes.c_int, [_vp] * 13 + [_f32, _i64, _i32, _vp]),
-    "rsb_bn_partials_finalize": (ctypes.c_int, [_vp, _i64] + [_vp] * 10 + [_i64, _i32, _f32, _f32, _i32, _vp]),
-    "rsb_bn_finalize": (ctypes.c_int, [_vp] * 10 + [_i32, _i64, _f32, _f32, _vp]),
-    "rsb_bn_apply": (ctypes.c_int, [_vp] * 5 + [_i64, _i32, _i32, _vp]),
-    "rsb_bn_backward": (ctypes.c_int, [_vp] * 13 + [_f32, _i64, _i32, _vp]),
+    "rsb_bn_partials_finalize": (ctypes.c_int, [_vp, _i64] + [_vp] * 10 + [_i64, _i32, _f32, _f32, _vp]),
     "rsb_relu_backward": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp]),
     "rsb_multi_axpy": (ctypes.c_int, [_vp, _i32, ctypes.c_float, _vp]),
     "rsb_maxpool_backward": (ctypes.c_int, [_vp, _vp, _vp, _vp] + [_i32] * 7 + [_vp]),
@@ -260,7 +254,6 @@ SIGNATURES = {
     "rsb_final_backward": (ctypes.c_int, [_vp] * 7 + [_f32, _i32, _i32, _i32, _vp]),
     "rsb_pack_weights": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp]),
     "rsb_pack_weights1": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp]),
-    "rsb_unpack_grads": (ctypes.c_int, [_vp, _vp, _vp, _i64, _f32, _vp]),
     "rsb_unpack_grads_gather": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp]),
     "rsb_wgrad_plan_create": (ctypes.c_int, [ctypes.POINTER(ConvDesc), _vp, _vp, ctypes.POINTER(_vp)]),
     "rsb_wgrad_plan_scratch_bytes": (_i64, [_vp]),

@@ -39,9 +39,9 @@ __device__ __forceinline__ void pdl_sync() {
 }
 
 template <typename... KArgs, typename... Args>
-static cudaError_t launch_chained(bool chained, void (*kern)(KArgs...), unsigned grid, unsigned block, cudaStream_t st, Args... args) {
+static cudaError_t launch_chained(void (*kern)(KArgs...), dim3 grid, unsigned block, cudaStream_t st, Args... args) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
+    cfg.gridDim = grid;
     cfg.blockDim = dim3(block);
     cfg.dynamicSmemBytes = 0;
     cfg.stream = st;
@@ -49,7 +49,7 @@ static cudaError_t launch_chained(bool chained, void (*kern)(KArgs...), unsigned
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = chained ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
@@ -72,10 +72,9 @@ __device__ __forceinline__ void store8(__half* p, const float (&v)[8]) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// per-channel sums over M rows of an NHWC fp16 tensor [M][C]; two fused reductions:
-//   KIND 0 (forward stats)   : s0 += z            s1 += z*z
-//   KIND 1 (BN backward)     : g = dy * (y > 0 or no mask); s0 += g ; s1 += g * z   (raw: consumers turn it into
-//                              sum g*zhat = (s1 - mean*s0) * invstd, which keeps mean / invstd out of the streaming loop)
+// per-channel sums of the BatchNorm backward over M rows of NHWC fp16 tensors [M][C]:
+//   g = dy * (y > 0 or no mask); s0 += g ; s1 += g * z   (raw: the epilogue turns it into sum g*zhat = (s1 - mean*s0) * invstd,
+//   which keeps mean / invstd out of the streaming loop)
 // 256 threads: C/8 threads cover one row (8 channels = 16 bytes each), 256/(C/8) rows per iteration, two iterations in
 // flight per thread. Block totals go to one of kRedSlots replicated fp64 accumulators (slot = block % kRedSlots) so that
 // at most blocks/kRedSlots atomics queue up on an address; consumers add the slots.
@@ -83,22 +82,23 @@ static constexpr int kRedSlots = 8;
 
 // Scratch layout (doubles): [kRedSlots][2][C] accumulators | 1 arrival counter | 1 pad | (as floats) 3*C coefficients.
 // The LAST block to finish (arrival counter) folds the slots and does the per-channel epilogue, so no extra launch is needed:
-//   KIND 0: BatchNorm finalize (mean / invstd / folded scale+shift, running statistics)      -- when tail.gamma != NULL
-//   KIND 1: dgamma / dbeta and the coefficients A, B, D of dz = A*g + B*z + D for bn_bwd_apply_kernel
+//   partial_reduce_kernel: BatchNorm finalize (mean / invstd / folded scale+shift, running statistics)
+//   channel_reduce_kernel: dgamma / dbeta and the coefficients A, B, D of dz = A*g + B*z + D for bn_bwd_apply_kernel
+// It then zeroes the accumulator slots and the arrival counter for the next call, so the scratch is zeroed once by the caller
+// and never by a memset launch.
 struct RedTail {
     const float* gamma;
     const float* beta;
     float* running_mean;
     float* running_var;
     int64_t* num_batches;
-    float* mean;    // KIND 0: out; KIND 1: in
-    float* invstd;  // KIND 0: out; KIND 1: in
+    float* mean;    // finalize: out; backward: in
+    float* invstd;  // finalize: out; backward: in
     float* scale;
     float* shift;
     float* dgamma;
     float* dbeta;
     float eps, momentum, inv_scale;
-    int self_clean;  // the last block leaves the accumulator slots and the arrival counter zeroed for the next call (no memset launch)
 };
 
 __device__ __forceinline__ double red_slots(const double* sums, int which, int c, int C) {
@@ -108,14 +108,22 @@ __device__ __forceinline__ double red_slots(const double* sums, int which, int c
     return t;
 }
 
+__device__ __forceinline__ void clear_slots(double* sums, int c, int C) {
+#pragma unroll
+    for (int sl = 0; sl < kRedSlots; ++sl) {
+        sums[(static_cast<int64_t>(sl) * 2 + 0) * C + c] = 0.0;
+        sums[(static_cast<int64_t>(sl) * 2 + 1) * C + c] = 0.0;
+    }
+}
+
 // ZMASK: the ReLU mask of a plain relu(bn(z)) output is re-derived from z instead of reading y: bn_apply_kernel rounds
 // o = fma(z, scale, shift) to fp16, and half(o) > 0 exactly when o > 2^-25 (round-to-nearest-even), so the mask is bit-identical.
 static constexpr float kHalfPositive = 0x1p-25f;
 
-template <int KIND, bool ZMASK = false>
+template <bool ZMASK>
 __global__ void __launch_bounds__(256, 2) channel_reduce_kernel(const __half* __restrict__ a, const __half* __restrict__ y, const __half* __restrict__ z,
                                                              double* __restrict__ sums, int64_t M, int C, const RedTail tail,
-                                                             const float* __restrict__ msc = nullptr, const float* __restrict__ msh = nullptr) {
+                                                             const float* __restrict__ msc, const float* __restrict__ msh) {
     __shared__ float sh0[256 * 8];
     __shared__ float sh1[256 * 8];
     pdl_sync();
@@ -138,14 +146,9 @@ __global__ void __launch_bounds__(256, 2) channel_reduce_kernel(const __half* __
     auto fold = [&](const float (&v)[8], const float (&zz)[8], const float (&yy)[8], bool masked) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            if (KIND == 0) {
-                acc0[i] += v[i];
-                acc1[i] = fmaf(v[i], v[i], acc1[i]);
-            } else {
-                const float g = (masked && !(yy[i] > 0.f)) ? 0.f : v[i];
-                acc0[i] += g;
-                acc1[i] = fmaf(g, zz[i], acc1[i]);
-            }
+            const float g = (masked && !(yy[i] > 0.f)) ? 0.f : v[i];
+            acc0[i] += g;
+            acc1[i] = fmaf(g, zz[i], acc1[i]);
         }
     };
     int64_t r = static_cast<int64_t>(blockIdx.x) * rows_per_iter + rsub;
@@ -167,23 +170,19 @@ __global__ void __launch_bounds__(256, 2) channel_reduce_kernel(const __half* __
         uint4 qa[4], qz[4], qy[4];
 #pragma unroll
         for (int u = 0; u < 4; ++u) qa[u] = raw(a + (r + u * step) * C + col);
-        if (KIND == 1) {
 #pragma unroll
-            for (int u = 0; u < 4; ++u) qz[u] = raw(z + (r + u * step) * C + col);
-            if (use_y) {
+        for (int u = 0; u < 4; ++u) qz[u] = raw(z + (r + u * step) * C + col);
+        if (use_y) {
 #pragma unroll
-                for (int u = 0; u < 4; ++u) qy[u] = raw(y + (r + u * step) * C + col);
-            }
+            for (int u = 0; u < 4; ++u) qy[u] = raw(y + (r + u * step) * C + col);
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
             float v0[8], z0[8], y0[8];
             cvt(qa[u], v0);
-            if (KIND == 1) {
-                cvt(qz[u], z0);
-                if (ZMASK) zmask(z0, y0);
-                else if (use_y) cvt(qy[u], y0);
-            }
+            cvt(qz[u], z0);
+            if (ZMASK) zmask(z0, y0);
+            else if (use_y) cvt(qy[u], y0);
             fold(v0, z0, y0, ZMASK || y != nullptr);
         }
     }
@@ -191,16 +190,14 @@ __global__ void __launch_bounds__(256, 2) channel_reduce_kernel(const __half* __
         float v0[8], v1[8], z0[8], z1[8], y0[8], y1[8];
         load8(a + r * C + col, v0);
         load8(a + (r + step) * C + col, v1);
-        if (KIND == 1) {
-            load8(z + r * C + col, z0);
-            load8(z + (r + step) * C + col, z1);
-            if (ZMASK) {
-                zmask(z0, y0);
-                zmask(z1, y1);
-            } else if (y) {
-                load8(y + r * C + col, y0);
-                load8(y + (r + step) * C + col, y1);
-            }
+        load8(z + r * C + col, z0);
+        load8(z + (r + step) * C + col, z1);
+        if (ZMASK) {
+            zmask(z0, y0);
+            zmask(z1, y1);
+        } else if (y) {
+            load8(y + r * C + col, y0);
+            load8(y + (r + step) * C + col, y1);
         }
         fold(v0, z0, y0, ZMASK || y != nullptr);
         fold(v1, z1, y1, ZMASK || y != nullptr);
@@ -208,11 +205,9 @@ __global__ void __launch_bounds__(256, 2) channel_reduce_kernel(const __half* __
     if (r < M) {
         float v0[8], z0[8], y0[8];
         load8(a + r * C + col, v0);
-        if (KIND == 1) {
-            load8(z + r * C + col, z0);
-            if (ZMASK) zmask(z0, y0);
-            else if (y) load8(y + r * C + col, y0);
-        }
+        load8(z + r * C + col, z0);
+        if (ZMASK) zmask(z0, y0);
+        else if (y) load8(y + r * C + col, y0);
         fold(v0, z0, y0, ZMASK || y != nullptr);
     }
 #pragma unroll
@@ -234,7 +229,6 @@ __global__ void __launch_bounds__(256, 2) channel_reduce_kernel(const __half* __
         atomicAdd(&s0[c], static_cast<double>(a0));
         atomicAdd(&s1[c], static_cast<double>(a1));
     }
-    if (tail.gamma == nullptr) return;
     // ---- last block: per-channel epilogue
     __shared__ bool is_last;
     __threadfence();
@@ -247,51 +241,27 @@ __global__ void __launch_bounds__(256, 2) channel_reduce_kernel(const __half* __
     if (!is_last) return;
     __threadfence();
     const double dM = static_cast<double>(M);
-    if (KIND == 0 && threadIdx.x == 0 && tail.num_batches) *tail.num_batches += 1;
     float* coef = reinterpret_cast<float*>(sums + static_cast<int64_t>(kRedSlots) * 2 * C + 2);
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         const double t0 = red_slots(sums, 0, c, C), t1 = red_slots(sums, 1, c, C);
-        if (KIND == 0) {
-            const double mean = t0 / dM;
-            double var = t1 / dM - mean * mean;
-            if (var < 0) var = 0;
-            const float invstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(tail.eps)));
-            const float sc = tail.gamma[c] * invstd;
-            tail.mean[c] = static_cast<float>(mean);
-            tail.invstd[c] = invstd;
-            tail.scale[c] = sc;
-            tail.shift[c] = tail.beta[c] - static_cast<float>(mean) * sc;
-            if (tail.running_mean) {
-                const double unbiased = dM > 1 ? var * dM / (dM - 1.0) : var;
-                tail.running_mean[c] = (1.f - tail.momentum) * tail.running_mean[c] + tail.momentum * static_cast<float>(mean);
-                tail.running_var[c] = (1.f - tail.momentum) * tail.running_var[c] + tail.momentum * static_cast<float>(unbiased);
-            }
-        } else {
-            const float is = tail.invstd[c], ga = tail.gamma[c], mu = tail.mean[c];
-            const double sgzh = (t1 - static_cast<double>(mu) * t0) * static_cast<double>(is);  // sum of g * zhat
-            tail.dgamma[c] = static_cast<float>(sgzh) * tail.inv_scale;
-            tail.dbeta[c] = static_cast<float>(t0) * tail.inv_scale;
-            const float mg = static_cast<float>(t0 / dM), mgz = static_cast<float>(sgzh / dM);
-            coef[c] = ga * is;                                        // A
-            coef[C + c] = -ga * is * is * mgz;                        // B
-            coef[2 * C + c] = -ga * is * mg + ga * is * is * mu * mgz;  // D
-        }
-        if (tail.self_clean) {
-#pragma unroll
-            for (int sl = 0; sl < kRedSlots; ++sl) {
-                sums[(static_cast<int64_t>(sl) * 2 + 0) * C + c] = 0.0;
-                sums[(static_cast<int64_t>(sl) * 2 + 1) * C + c] = 0.0;
-            }
-        }
+        const float is = tail.invstd[c], ga = tail.gamma[c], mu = tail.mean[c];
+        const double sgzh = (t1 - static_cast<double>(mu) * t0) * static_cast<double>(is);  // sum of g * zhat
+        tail.dgamma[c] = static_cast<float>(sgzh) * tail.inv_scale;
+        tail.dbeta[c] = static_cast<float>(t0) * tail.inv_scale;
+        const float mg = static_cast<float>(t0 / dM), mgz = static_cast<float>(sgzh / dM);
+        coef[c] = ga * is;                                        // A
+        coef[C + c] = -ga * is * is * mgz;                        // B
+        coef[2 * C + c] = -ga * is * mg + ga * is * is * mu * mgz;  // D
+        clear_slots(sums, c, C);
     }
-    if (tail.self_clean && threadIdx.x == 0) *reinterpret_cast<unsigned*>(sums + static_cast<int64_t>(kRedSlots) * 2 * C) = 0u;
+    if (threadIdx.x == 0) *reinterpret_cast<unsigned*>(sums + static_cast<int64_t>(kRedSlots) * 2 * C) = 0u;
 }
 
 // ------------------------------------------------------------------------------------------------
 // Batch statistics from the per-quarter-tile partial sums a STATS convolution wrote (rsb_conv_desc.stats): P is an fp32
 // matrix [R][L], L = 2*C (row = one 32-pixel quarter of a tile: C sums, then C sums of squares). Column sums go to the same
-// replicated fp64 accumulators as channel_reduce_kernel<0> ([slot][2][C] == [slot][L]) and the last block runs the same
-// BatchNorm finalize, so the op reads 1/8 of the bytes of z instead of all of z.
+// replicated fp64 accumulators as channel_reduce_kernel ([slot][2][C] == [slot][L]) and the last block runs the BatchNorm
+// finalize, so the op reads 1/8 of the bytes of z instead of all of z.
 __global__ void __launch_bounds__(256) partial_reduce_kernel(const float* __restrict__ P, double* __restrict__ sums, int64_t R, int L, int C, int64_t M,
                                                             const RedTail tail) {
     __shared__ float4 sh[256];
@@ -335,7 +305,7 @@ __global__ void __launch_bounds__(256) partial_reduce_kernel(const float* __rest
         atomicAdd(&s[2], static_cast<double>(t.z));
         atomicAdd(&s[3], static_cast<double>(t.w));
     }
-    // ---- last block (of the whole 2-D grid): BatchNorm finalize, as in channel_reduce_kernel<0>
+    // ---- last block (of the whole 2-D grid): BatchNorm finalize
     __shared__ bool is_last;
     __threadfence();
     __syncthreads();
@@ -364,39 +334,9 @@ __global__ void __launch_bounds__(256) partial_reduce_kernel(const float* __rest
             tail.running_mean[c] = (1.f - tail.momentum) * tail.running_mean[c] + tail.momentum * static_cast<float>(mean);
             tail.running_var[c] = (1.f - tail.momentum) * tail.running_var[c] + tail.momentum * static_cast<float>(unbiased);
         }
-        if (tail.self_clean) {
-#pragma unroll
-            for (int sl = 0; sl < kRedSlots; ++sl) {
-                sums[(static_cast<int64_t>(sl) * 2 + 0) * C + c] = 0.0;
-                sums[(static_cast<int64_t>(sl) * 2 + 1) * C + c] = 0.0;
-            }
-        }
+        clear_slots(sums, c, C);
     }
-    if (tail.self_clean && threadIdx.x == 0) *reinterpret_cast<unsigned*>(sums + static_cast<int64_t>(kRedSlots) * 2 * C) = 0u;
-}
-
-// mean / invstd / folded scale+shift from the batch sums, running-stat update (momentum, unbiased variance)
-__global__ void bn_finalize_kernel(const double* __restrict__ sums, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, float* __restrict__ running_mean, float* __restrict__ running_var,
-                                   int64_t* __restrict__ num_batches, float* __restrict__ mean_out, float* __restrict__ invstd_out,
-                                   float* __restrict__ scale_out, float* __restrict__ shift_out, int C, double M, float eps, float momentum) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c == 0 && num_batches) *num_batches += 1;
-    if (c >= C) return;
-    const double mean = red_slots(sums, 0, c, C) / M;
-    double var = red_slots(sums, 1, c, C) / M - mean * mean;
-    if (var < 0) var = 0;
-    const float invstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
-    const float sc = gamma[c] * invstd;
-    mean_out[c] = static_cast<float>(mean);
-    invstd_out[c] = invstd;
-    scale_out[c] = sc;
-    shift_out[c] = beta[c] - static_cast<float>(mean) * sc;
-    if (running_mean) {
-        const double unbiased = M > 1 ? var * M / (M - 1.0) : var;
-        running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * static_cast<float>(mean);
-        running_var[c] = (1.f - momentum) * running_var[c] + momentum * static_cast<float>(unbiased);
-    }
+    if (threadIdx.x == 0) *reinterpret_cast<unsigned*>(sums + static_cast<int64_t>(kRedSlots) * 2 * C) = 0u;
 }
 
 // y = relu?(z * scale + shift (+ res)). The grid stride (blocks * 256) is a multiple of C/8 (C/8 divides 256), so every
@@ -802,8 +742,8 @@ __global__ void f64_to_f32_kernel(const double* __restrict__ src, float* __restr
 // ------------------------------------------------------------------------------------------------
 // fp32 master weights -> fp16 packed operand matrices, and packed fp32 gradients -> fp32 OIHW gradients.
 // A packed matrix is [rows][K]; `map` gives, for every packed element, up to 4 source indices into the OIHW tensor
-// (-1 = none): forward packs gather one element, the upsample phases sum up to four taps. The same map drives the
-// gradient scatter (packed gradient element added to each of its sources).
+// (-1 = none): forward packs gather one element, the upsample phases sum up to four taps. The inverse of the same map drives
+// the gradient un-pack (each OIHW element gathers the packed gradient elements it was a source of).
 __global__ void pack_gather_kernel(const float* __restrict__ src, const int32_t* __restrict__ map, __half* __restrict__ dst, int64_t n) {
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int4 m = __ldg(reinterpret_cast<const int4*>(map) + i);
@@ -830,21 +770,9 @@ __global__ void pack_gather1_kernel(const float* __restrict__ src, const int32_t
     }
 }
 
-__global__ void unpack_scatter_kernel(const float* __restrict__ packed_grad, const int32_t* __restrict__ map, float* __restrict__ grad,
-                                      int64_t n, float mul) {
-    for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int4 m = __ldg(reinterpret_cast<const int4*>(map) + i);
-        const float g = packed_grad[i] * mul;
-        if (m.x >= 0) atomicAdd(&grad[m.x], g);
-        if (m.y >= 0) atomicAdd(&grad[m.y], g);
-        if (m.z >= 0) atomicAdd(&grad[m.z], g);
-        if (m.w >= 0) atomicAdd(&grad[m.w], g);
-    }
-}
-
-// Deterministic form of the same scatter: one thread per OIHW gradient element, which GATHERS its (at most four) packed
-// contributions in index order -- the nearest-x2 phases route every 3x3 weight into four packed elements, and adding those with
-// atomics made the last bits of the decoder gradients depend on the thread schedule.
+// The transpose of the same map, without atomics: one thread per OIHW gradient element, which GATHERS its (at most four) packed
+// contributions in index order. The nearest-x2 phases route every 3x3 weight into four packed elements; adding those with atomics
+// would make the last bits of the decoder gradients depend on the thread schedule.
 __global__ void unpack_gather_kernel(const float* __restrict__ packed_grad, const int32_t* __restrict__ dst_idx, const int32_t* __restrict__ inv,
                                      float* __restrict__ grad, int64_t n, float mul) {
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
@@ -880,72 +808,12 @@ using namespace rsb;
 
 static bool bad_c(int C) { return C <= 0 || (C % 8) || (C > 2048) || (256 % (C / 8 > 256 ? 256 : C / 8)); }
 
-extern "C" int rsb_bn_stats(const void* z, double* sums, int64_t M, int32_t C, void* stream) {
-    if (!z || !sums || M <= 0 || bad_c(C) || C < 64) return set_error(RSB_E_INVALID, "bn_stats: bad arguments (C in 64..2048, power of two)");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * (2 * C * kRedSlots + 2), st);
-    if (e != cudaSuccess) return set_cuda_error(e, "bn_stats memset");
-    RedTail tail = {};
-    channel_reduce_kernel<0><<<reduce_blocks(M, C), 256, 0, st>>>(static_cast<const __half*>(z), nullptr, nullptr, sums, M, C, tail);
-    RSB_LAUNCH_CHECK("bn_stats launch");
-    return RSB_OK;
-}
-
-static int bn_stats_finalize_impl(const void* z, double* sums, const float* gamma, const float* beta, float* running_mean, float* running_var,
-                                  int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int64_t M, int32_t C, float eps,
-                                  float momentum, void* stream, bool chained) {
-    if (!z || !sums || !gamma || !beta || !mean || !invstd || !scale || !shift || M <= 0 || bad_c(C) || C < 64)
-        return set_error(RSB_E_INVALID, "bn_stats_finalize: bad arguments (C in 64..2048, power of two)");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (!chained) {
-        cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * (2 * C * kRedSlots + 2), st);
-        if (e != cudaSuccess) return set_cuda_error(e, "bn_stats_finalize memset");
-    }
-    RedTail tail = {};
-    tail.gamma = gamma;
-    tail.beta = beta;
-    tail.running_mean = running_mean;
-    tail.running_var = running_var;
-    tail.num_batches = num_batches;
-    tail.mean = mean;
-    tail.invstd = invstd;
-    tail.scale = scale;
-    tail.shift = shift;
-    tail.eps = eps;
-    tail.momentum = momentum;
-    tail.self_clean = chained ? 1 : 0;
-    cudaError_t e = launch_chained(chained, channel_reduce_kernel<0, false>, reduce_blocks(M, C), 256, st, static_cast<const __half*>(z),
-                                   static_cast<const __half*>(nullptr), static_cast<const __half*>(nullptr), sums, M, static_cast<int>(C), tail,
-                                   static_cast<const float*>(nullptr), static_cast<const float*>(nullptr));
-    if (e != cudaSuccess) return set_cuda_error(e, "bn_stats_finalize launch");
-    return RSB_OK;
-}
-
-extern "C" int rsb_bn_stats_finalize(const void* z, double* sums, const float* gamma, const float* beta, float* running_mean, float* running_var,
-                                     int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int64_t M, int32_t C, float eps,
-                                     float momentum, void* stream) {
-    return bn_stats_finalize_impl(z, sums, gamma, beta, running_mean, running_var, num_batches, mean, invstd, scale, shift, M, C, eps, momentum, stream,
-                                  false);
-}
-
-extern "C" int rsb_bn_stats_finalize_chained(const void* z, double* sums, const float* gamma, const float* beta, float* running_mean,
-                                             float* running_var, int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift,
-                                             int64_t M, int32_t C, float eps, float momentum, void* stream) {
-    return bn_stats_finalize_impl(z, sums, gamma, beta, running_mean, running_var, num_batches, mean, invstd, scale, shift, M, C, eps, momentum, stream,
-                                  true);
-}
-
 extern "C" int rsb_bn_partials_finalize(const float* partials, int64_t rows, double* sums, const float* gamma, const float* beta, float* running_mean,
                                         float* running_var, int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int64_t M,
-                                        int32_t C, float eps, float momentum, int32_t chained, void* stream) {
+                                        int32_t C, float eps, float momentum, void* stream) {
     if (!partials || rows <= 0 || !sums || !gamma || !beta || !mean || !invstd || !scale || !shift || M <= 0 || bad_c(C) || C < 32 ||
         (reinterpret_cast<uintptr_t>(partials) & 15))
         return set_error(RSB_E_INVALID, "bn_partials_finalize: bad arguments (C in 32..2048, power of two; partials 16B aligned)");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (!chained) {
-        cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * (2 * C * kRedSlots + 2), st);
-        if (e != cudaSuccess) return set_cuda_error(e, "bn_partials_finalize memset");
-    }
     RedTail tail = {};
     tail.gamma = gamma;
     tail.beta = beta;
@@ -958,7 +826,6 @@ extern "C" int rsb_bn_partials_finalize(const float* partials, int64_t rows, dou
     tail.shift = shift;
     tail.eps = eps;
     tail.momentum = momentum;
-    tail.self_clean = chained ? 1 : 0;
     const int L = 2 * C;
     const int tpr = L / 4 < 256 ? L / 4 : 256;
     const int colblocks = L / (tpr * 4);
@@ -967,63 +834,30 @@ extern "C" int rsb_bn_partials_finalize(const float* partials, int64_t rows, dou
     const int64_t cap = (2 * num_sms() + colblocks - 1) / colblocks;
     if (bx > cap) bx = cap;
     if (bx < 1) bx = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned>(bx), static_cast<unsigned>(colblocks));
-    cfg.blockDim = dim3(256);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = chained ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, partial_reduce_kernel, partials, sums, rows, L, static_cast<int>(C), M, tail);
+    cudaError_t e = launch_chained(partial_reduce_kernel, dim3(static_cast<unsigned>(bx), static_cast<unsigned>(colblocks)), 256,
+                                   static_cast<cudaStream_t>(stream), partials, sums, rows, L, static_cast<int>(C), M, tail);
     if (e != cudaSuccess) return set_cuda_error(e, "bn_partials_finalize launch");
     return RSB_OK;
 }
 
-extern "C" int rsb_bn_finalize(const double* sums, const float* gamma, const float* beta, float* running_mean, float* running_var,
-                               int64_t* num_batches, float* mean, float* invstd, float* scale, float* shift, int32_t C, int64_t M,
-                               float eps, float momentum, void* stream) {
-    if (!sums || !gamma || !beta || !mean || !invstd || !scale || !shift || C <= 0 || M <= 0) return set_error(RSB_E_INVALID, "bn_finalize: bad arguments");
-    bn_finalize_kernel<<<(C + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(sums, gamma, beta, running_mean, running_var,
-                                                                                   num_batches, mean, invstd, scale, shift, C,
-                                                                                   static_cast<double>(M), eps, momentum);
-    RSB_LAUNCH_CHECK("bn_finalize launch");
-    return RSB_OK;
-}
-
-static int bn_apply_impl(const void* z, const float* scale, const float* shift, const void* residual, void* y, int64_t M, int32_t C, int32_t relu,
-                         void* stream, bool chained) {
+extern "C" int rsb_bn_apply_chained(const void* z, const float* scale, const float* shift, const void* residual, void* y, int64_t M, int32_t C,
+                                    int32_t relu, void* stream) {
     if (!z || !scale || !shift || !y || M <= 0 || C <= 0 || (C % 8)) return set_error(RSB_E_INVALID, "bn_apply: bad arguments");
-    cudaError_t e = launch_chained(chained, bn_apply_kernel, tr_blocks(M * (C / 8), 256), 256, static_cast<cudaStream_t>(stream),
+    cudaError_t e = launch_chained(bn_apply_kernel, tr_blocks(M * (C / 8), 256), 256, static_cast<cudaStream_t>(stream),
                                    static_cast<const __half*>(z), scale, shift, static_cast<const __half*>(residual), static_cast<__half*>(y), M,
                                    static_cast<int>(C), static_cast<int>(relu));
     if (e != cudaSuccess) return set_cuda_error(e, "bn_apply launch");
     return RSB_OK;
 }
 
-extern "C" int rsb_bn_apply(const void* z, const float* scale, const float* shift, const void* residual, void* y, int64_t M, int32_t C,
-                            int32_t relu, void* stream) {
-    return bn_apply_impl(z, scale, shift, residual, y, M, C, relu, stream, false);
-}
-
-extern "C" int rsb_bn_apply_chained(const void* z, const float* scale, const float* shift, const void* residual, void* y, int64_t M, int32_t C,
-                                    int32_t relu, void* stream) {
-    return bn_apply_impl(z, scale, shift, residual, y, M, C, relu, stream, true);
-}
-
-static int bn_backward_impl(const void* dy, const void* y, const void* z, const float* mean, const float* invstd, const float* gamma,
-                            const float* mask_scale, const float* mask_shift, double* sums, void* dz, void* g_out, float* dgamma, float* dbeta,
-                            float inv_loss_scale, int64_t M, int32_t C, void* stream, bool chained) {
+extern "C" int rsb_bn_backward_chained(const void* dy, const void* y, const void* z, const float* mean, const float* invstd, const float* gamma,
+                                       const float* mask_scale, const float* mask_shift, double* sums, void* dz, void* g_out, float* dgamma,
+                                       float* dbeta, float inv_loss_scale, int64_t M, int32_t C, void* stream) {
     if (!dy || !z || !mean || !invstd || !gamma || !sums || !dz || !dgamma || !dbeta || M <= 0 || bad_c(C) || C < 64)
         return set_error(RSB_E_INVALID, "bn_backward: bad arguments");
     if ((mask_scale != nullptr) != (mask_shift != nullptr) || (mask_scale && y))
         return set_error(RSB_E_INVALID, "bn_backward: pass either y, or mask_scale + mask_shift, or neither");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (!chained) {
-        cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * (2 * C * kRedSlots + 2), st);
-        if (e != cudaSuccess) return set_cuda_error(e, "bn_backward memset");
-    }
     RedTail tail = {};
     tail.gamma = gamma;
     tail.mean = const_cast<float*>(mean);
@@ -1031,7 +865,6 @@ static int bn_backward_impl(const void* dy, const void* y, const void* z, const 
     tail.dgamma = dgamma;
     tail.dbeta = dbeta;
     tail.inv_scale = inv_loss_scale;
-    tail.self_clean = chained ? 1 : 0;
     const __half* dyh = static_cast<const __half*>(dy);
     const __half* yh = static_cast<const __half*>(y);
     const __half* zh = static_cast<const __half*>(z);
@@ -1041,31 +874,19 @@ static int bn_backward_impl(const void* dy, const void* y, const void* z, const 
     const float* nullf = nullptr;
     cudaError_t e;
     if (mask_scale) {
-        e = launch_chained(chained, channel_reduce_kernel<1, true>, reduce_blocks(M, C), 256, st, dyh, nullh, zh, sums, M, static_cast<int>(C), tail, mask_scale,
+        e = launch_chained(channel_reduce_kernel<true>, reduce_blocks(M, C), 256, st, dyh, nullh, zh, sums, M, static_cast<int>(C), tail, mask_scale,
                            mask_shift);
         if (e == cudaSuccess)
-            e = launch_chained(chained, bn_bwd_apply_kernel<true>, ablocks, 256, st, dyh, nullh, zh, coef, static_cast<__half*>(dz), static_cast<__half*>(g_out),
+            e = launch_chained(bn_bwd_apply_kernel<true>, ablocks, 256, st, dyh, nullh, zh, coef, static_cast<__half*>(dz), static_cast<__half*>(g_out),
                                M, static_cast<int>(C), mask_scale, mask_shift);
     } else {
-        e = launch_chained(chained, channel_reduce_kernel<1, false>, reduce_blocks(M, C), 256, st, dyh, yh, zh, sums, M, static_cast<int>(C), tail, nullf, nullf);
+        e = launch_chained(channel_reduce_kernel<false>, reduce_blocks(M, C), 256, st, dyh, yh, zh, sums, M, static_cast<int>(C), tail, nullf, nullf);
         if (e == cudaSuccess)
-            e = launch_chained(chained, bn_bwd_apply_kernel<false>, ablocks, 256, st, dyh, yh, zh, coef, static_cast<__half*>(dz), static_cast<__half*>(g_out),
+            e = launch_chained(bn_bwd_apply_kernel<false>, ablocks, 256, st, dyh, yh, zh, coef, static_cast<__half*>(dz), static_cast<__half*>(g_out),
                                M, static_cast<int>(C), nullf, nullf);
     }
     if (e != cudaSuccess) return set_cuda_error(e, "bn_backward launch");
     return RSB_OK;
-}
-
-extern "C" int rsb_bn_backward(const void* dy, const void* y, const void* z, const float* mean, const float* invstd, const float* gamma,
-                               const float* mask_scale, const float* mask_shift, double* sums, void* dz, void* g_out, float* dgamma, float* dbeta,
-                               float inv_loss_scale, int64_t M, int32_t C, void* stream) {
-    return bn_backward_impl(dy, y, z, mean, invstd, gamma, mask_scale, mask_shift, sums, dz, g_out, dgamma, dbeta, inv_loss_scale, M, C, stream, false);
-}
-
-extern "C" int rsb_bn_backward_chained(const void* dy, const void* y, const void* z, const float* mean, const float* invstd, const float* gamma,
-                                       const float* mask_scale, const float* mask_shift, double* sums, void* dz, void* g_out, float* dgamma,
-                                       float* dbeta, float inv_loss_scale, int64_t M, int32_t C, void* stream) {
-    return bn_backward_impl(dy, y, z, mean, invstd, gamma, mask_scale, mask_shift, sums, dz, g_out, dgamma, dbeta, inv_loss_scale, M, C, stream, true);
 }
 
 extern "C" int rsb_relu_backward(const void* a, const void* b, const void* y, void* out, int64_t n, void* stream) {
@@ -1136,13 +957,6 @@ extern "C" int rsb_pack_weights1(const float* src, const int32_t* map1, void* ds
         return set_error(RSB_E_INVALID, "pack_weights1: bad arguments (n a multiple of 8, map and dst 16B aligned)");
     pack_gather1_kernel<<<tr_blocks(n / 8, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(src, map1, static_cast<__half*>(dst), n / 8);
     RSB_LAUNCH_CHECK("pack_weights1 launch");
-    return RSB_OK;
-}
-
-extern "C" int rsb_unpack_grads(const float* packed_grad, const int32_t* map4, float* grad, int64_t n, float mul, void* stream) {
-    if (!packed_grad || !map4 || !grad || n <= 0) return set_error(RSB_E_INVALID, "unpack_grads: bad arguments");
-    unpack_scatter_kernel<<<tr_blocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(packed_grad, map4, grad, n, mul);
-    RSB_LAUNCH_CHECK("unpack_grads launch");
     return RSB_OK;
 }
 

@@ -10,7 +10,8 @@
 // Work item = (128 output channels) x (phase) x (group of <= 4 consecutive 64-wide K blocks) x (slice of the pixel tiles).
 // Per 128-pixel tile: one dY box (2 x 16 KB) + one X box per K block (16 KB each) by TMA; consumer warpgroup g issues
 // 8 MMAs (M64 x N<=256 x K16) for output channels [64 g, 64 g + 64) into register accumulators. Epilogue: plain fp32 stores
-// or fp32 reductions into the packed gradient (split-K over pixel slices).
+// into the packed gradient, or, split-K over pixel slices, into the slice's partial gradient in a scratch buffer, which
+// wgrad_reduce_kernel adds up in slice order (bit-identical from run to run).
 
 #include <string.h>
 
@@ -47,8 +48,8 @@ struct alignas(64) WgradKParams {
     int32_t Cout;
     int64_t K;  // packed row length = 64 * kblocks
     float* dw;  // [phases*Cout][K] fp32
-    // deterministic split-K: slice s stores its partial gradient to partial + s * slice_stride (plain stores), and
-    // wgrad_reduce_kernel adds the slices in index order. NULL: fp32 atomic adds straight into dw (order-dependent last bits).
+    // split-K (slices > 1): slice s stores its partial gradient to partial + s * slice_stride, and wgrad_reduce_kernel adds
+    // the slices in index order. Set by rsb_wgrad_plan_set_scratch; a single slice stores straight into dw.
     float* partial;
     int64_t slice_stride;
 };
@@ -178,9 +179,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
                 case 3: run(std::integral_constant<int, 192>{}); break;
                 default: run(std::integral_constant<int, 256>{}); break;
             }
-            // one writer per element when there is a single slice or a partial buffer per slice: plain stores, no atomics
-            const bool plain = p.slices == 1 || p.partial != nullptr;
-            float* dbase = (p.partial != nullptr && p.slices > 1) ? p.partial + static_cast<int64_t>(it.slice) * p.slice_stride : p.dw;
+            // one writer per element: dw itself for a single slice, else this slice's partial buffer
+            float* dbase = p.slices > 1 ? p.partial + static_cast<int64_t>(it.slice) * p.slice_stride : p.dw;
             if (t_lo < p.ptiles) {
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
@@ -190,9 +190,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
 #pragma unroll
                     for (int j = 0; j < kWgGroup * 8; ++j) {
                         if (j < nkb * 8) {
-                            const float a = acc[4 * j + 2 * hh], b = acc[4 * j + 2 * hh + 1];
-                            if (plain) *reinterpret_cast<float2*>(drow + 8 * j + cq) = make_float2(a, b);
-                            else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(drow + 8 * j + cq), "f"(a), "f"(b) : "memory");
+                            *reinterpret_cast<float2*>(drow + 8 * j + cq) = make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
                         }
                     }
                 }
@@ -300,7 +298,7 @@ extern "C" int rsb_wgrad_plan_create(const rsb_conv_desc* d, const void* dy, flo
     kp.dw = dw_packed;
     // split-K over slices of the pixel tiles: pick the slice count that minimises rounds x (tiles per item + epilogue),
     // rounds = ceil(items / SMs) of the persistent grid (e.g. 160 items on 132 SMs would run two rounds for 28 extra items);
-    // every slice adds a full copy of the gradient tile (128 x 256 fp32 reductions ~ 8 stage times) to the traffic
+    // every slice adds a full copy of the gradient tile (128 x 256 fp32 partials ~ 8 stage times) to the traffic
     const int sms = num_sms();
     const int base_items = kp.co_blocks * kp.phases * kp.kgroups;
     int64_t best_cost = -1;
@@ -332,9 +330,9 @@ extern "C" int64_t rsb_wgrad_plan_scratch_bytes(const rsb_wgrad_plan* plan) {
 extern "C" int rsb_wgrad_plan_set_scratch(rsb_wgrad_plan* plan, float* scratch, int64_t scratch_bytes) {
     if (!plan) return set_error(RSB_E_INVALID, "wgrad: null plan");
     const int64_t need = rsb_wgrad_plan_scratch_bytes(plan);
-    if (need == 0) return RSB_OK;  // a single slice writes every element exactly once: already deterministic
+    if (need == 0) return RSB_OK;  // a single slice writes every element of dw exactly once
     if (!scratch || scratch_bytes < need || (reinterpret_cast<uintptr_t>(scratch) & 15))
-        return set_error(RSB_E_INVALID, "wgrad: deterministic split-K needs a 16B-aligned scratch of >= %lld bytes", (long long)need);
+        return set_error(RSB_E_INVALID, "wgrad: split-K needs a 16B-aligned scratch of >= %lld bytes", (long long)need);
     plan->kp.partial = scratch;
     plan->kp.slice_stride = plan->dw_bytes / 4;
     return RSB_OK;
@@ -344,6 +342,8 @@ extern "C" void rsb_wgrad_plan_destroy(rsb_wgrad_plan* plan) { delete plan; }
 
 extern "C" int rsb_wgrad_run(const rsb_wgrad_plan* plan, void* stream_) {
     if (!plan) return set_error(RSB_E_INVALID, "wgrad: null plan");
+    if (plan->kp.slices > 1 && plan->kp.partial == nullptr)
+        return set_error(RSB_E_INVALID, "wgrad: a split-K plan (%d slices) needs its scratch from rsb_wgrad_plan_set_scratch", plan->kp.slices);
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     static bool attr_set[64] = {};  // per device: one process may drive several GPUs
     int dev = 0;
@@ -353,16 +353,10 @@ extern "C" int rsb_wgrad_run(const rsb_wgrad_plan* plan, void* stream_) {
         if (e != cudaSuccess) return set_cuda_error(e, "cudaFuncSetAttribute(wgrad)");
         attr_set[dev] = true;
     }
-    const bool atomics = plan->kp.slices > 1 && plan->kp.partial == nullptr;
-    cudaError_t e = cudaSuccess;
-    if (atomics) {  // the plain-store paths write every element of their destination
-        e = cudaMemsetAsync(plan->kp.dw, 0, plan->dw_bytes, stream);
-        if (e != cudaSuccess) return set_cuda_error(e, "wgrad memset");
-    }
     wgrad_tc_kernel<<<plan->grid, kWgThreads, kWgSmem, stream>>>(plan->kp);
-    e = cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_cuda_error(e, "wgrad_tc_kernel launch");
-    if (plan->kp.slices > 1 && plan->kp.partial != nullptr) {
+    if (plan->kp.slices > 1) {
         const int64_t n4 = plan->dw_bytes / 16;
         int blocks = static_cast<int>((n4 + 255) / 256);
         if (blocks > 8 * num_sms()) blocks = 8 * num_sms();

@@ -4,10 +4,12 @@ Replaces what `outputs = net(images); loss.backward()` does in the reference's h
 (robosat/tools/train.py:180,186) for `UNet` (robosat/unet.py:110-141) with train-mode BatchNorm (torchvision resnet50):
 
   forward   per conv: fp32 master weights -> fp16 packed (rsb_pack_weights) -> wgmma conv (raw output z)
-            -> batch statistics (rsb_bn_stats / rsb_bn_finalize, running stats updated) -> y = relu(bn(z) (+ identity))
+            (its epilogue also writes per-tile BatchNorm partial sums) -> batch statistics from those partials
+            (rsb_bn_partials_finalize, running stats updated) -> y = relu(bn(z) (+ identity)) (rsb_bn_apply_chained)
             decoder convs have no BN: y = relu(conv) in the conv epilogue; final 1x1 conv is its own small kernel
-  backward  per conv: BN / ReLU backward (rsb_bn_backward, rsb_relu_backward) -> weight gradient on tensor cores in the
-            forward's packed layout (rsb_wgrad_*) -> rsb_unpack_grads to OIHW fp32 -> input gradient = the SAME conv
+  backward  per conv: BN / ReLU backward (rsb_bn_backward_chained, rsb_relu_backward) -> weight gradient on tensor cores in the
+            forward's packed layout (rsb_wgrad_*, deterministic split-K) -> rsb_unpack_grads_gather to OIHW fp32 -> input
+            gradient = the SAME conv
             kernel with transposed / flipped packed weights (strided convs and the fused upsample become 4-phase scatters,
             concat becomes one launch per source, fan-in sums ride on the kernel's residual input)
 
@@ -26,10 +28,7 @@ import torch
 from robosat_b200 import _lib
 from robosat_b200._lib import ConvSrc
 
-# BatchNorm kernels chained by programmatic dependent launch, accumulators cleaned by the kernels themselves (no memset launches)
 TRAIN_GRAPH = os.environ.get("RSB_TRAIN_GRAPH", "1") == "1"  # forward / backward op lists replayed from CUDA graphs
-CONV_STATS = os.environ.get("RSB_CONV_STATS", "1") == "1"  # BatchNorm batch sums from the conv epilogue
-BN_CHAINED = os.environ.get("RSB_BN_CHAINED", "1") == "1"  # chained BatchNorm finalize / apply kernels (0: separate passes)
 from robosat_b200.engine import ConvOp, _src_dense, _src_parity, make_conv_desc
 
 RESNET50_BLOCKS = (3, 4, 6, 3)
@@ -40,7 +39,7 @@ _UP_GROUPS = {0: ((0,), (1, 2)), 1: ((0, 1), (2,))}  # rows of the 3x3 kernel su
 
 # --------------------------------------------------------------------------------------------------
 # index maps: packed element -> up to 4 flat OIHW source indices (-1 = none). One map drives rsb_pack_weights
-# (gather + sum) and, for forward layouts, rsb_unpack_grads (scatter-add).
+# (gather + sum) and, inverted by invert_unpack_map, rsb_unpack_grads_gather for forward layouts.
 # --------------------------------------------------------------------------------------------------
 def _flat_index(shape):
     return np.arange(int(np.prod(shape)), dtype=np.int64).reshape(shape)
@@ -148,6 +147,26 @@ def map_window3_fwd(shape):
     return _map4(m)
 
 
+def invert_unpack_map(gmap):
+    """[n, 4] int32 pack map (packed element -> its <= 4 OIHW sources, -1 = none) -> (dst_idx, inv4) for rsb_unpack_grads_gather:
+    dst_idx [u] int32 lists every OIHW element that is a source at least once, in ascending order, and inv4 [u, 4] int32 its
+    packed elements in ascending order (-1 = none). Every gradient element then gathers its contributions in a fixed order."""
+    flat = gmap.reshape(-1).long()
+    valid = flat >= 0
+    src = flat[valid]
+    pk = (torch.arange(flat.numel(), device=gmap.device) // 4)[valid]
+    order = torch.argsort(src, stable=True)
+    src, pk = src[order], pk[order]
+    uniq, counts = torch.unique_consecutive(src, return_counts=True)
+    assert int(counts.max()) <= 4, "a weight receives more than 4 packed gradient contributions"
+    start = torch.cumsum(counts, 0) - counts
+    gid = torch.repeat_interleave(torch.arange(uniq.numel(), device=gmap.device), counts)
+    rank = torch.arange(src.numel(), device=gmap.device) - start[gid]
+    inv = torch.full((uniq.numel(), 4), -1, dtype=torch.int32, device=gmap.device)
+    inv[gid, rank] = pk.int()
+    return uniq.int().contiguous(), inv.contiguous()
+
+
 class Unit:
     """One convolution of the network with everything its forward and backward need."""
 
@@ -179,6 +198,8 @@ class UNetTrainEngine:
         self._grads_flat, self._grad_offset, self._unpack_all = None, {}, None
         self._keep = []
         self._pool_scratch = {}  # max-pool backward: one argmax byte per pooled element
+        self._wgrad_plans = []   # every weight-gradient plan, for moving them to a grown split-K scratch
+        self._wgrad_scratch = None
         self._accum_tables = {}
         self.grads = OrderedDict()
         self.units = OrderedDict()
@@ -239,7 +260,7 @@ class UNetTrainEngine:
                   out_offset=0, residual=None, stats=False, stats_slot=0):
         """forward conv (raw output unless relu=True) + its weight-gradient plan. stats=True (a conv feeding BatchNorm): the
         epilogue also writes the per-quarter-tile column sums / sums of squares that rsb_bn_partials_finalize folds, so the
-        batch statistics do not re-read z (RSB_CONV_STATS=0 keeps the separate reduction over z)."""
+        batch statistics do not re-read z."""
         u = Unit(name)
         u.wname = wname
         w = self.params[wname]
@@ -250,7 +271,7 @@ class UNetTrainEngine:
         u.desc = make_conv_desc(srcs, segs, wp, None, cout, phases, tile_space, out, out_pitches, out_scale=out_scale, relu=relu,
                                 out_offset_elems=out_offset, residual=residual)
         u.stats, u.stats_rows = None, 0
-        if stats and CONV_STATS:
+        if stats:
             d = u.desc
             rows = 4 * (-(-d.Wt // d.TW)) * (-(-d.Ht // d.TH)) * (-(-d.Nt // d.TN))
             need = rows * 2 * cout
@@ -275,15 +296,13 @@ class UNetTrainEngine:
         return u
 
     def _wgrad_scratch_for(self, plan):
-        """Deterministic split-K (default; RSB_WGRAD_DETERMINISTIC=0 restores fp32 atomics): one scratch for the per-slice partial
-        gradients, shared by every wgrad plan of the engine (launches are stream ordered) and grown to the largest request."""
-        if os.environ.get("RSB_WGRAD_DETERMINISTIC", "1") == "0":
-            return
+        """Deterministic split-K: one scratch for the per-slice partial gradients, shared by every wgrad plan of the engine
+        (launches are stream ordered) and grown to the largest request."""
         lib = _lib.load()
-        plans = self.__dict__.setdefault("_wgrad_plans", [])
+        plans = self._wgrad_plans
         plans.append(plan)
         need = int(lib.rsb_wgrad_plan_scratch_bytes(plan))
-        buf = self.__dict__.get("_wgrad_scratch")
+        buf = self._wgrad_scratch
         if need and (buf is None or buf.numel() * 4 < need):
             buf = self._wgrad_scratch = torch.empty((need + 3) // 4, dtype=torch.float32, device=self.device)
             for pl in plans[:-1]:  # plans created earlier move to the larger buffer
@@ -308,10 +327,11 @@ class UNetTrainEngine:
         op = self._conv_op(name, desc)
         return [("conv", op)]
 
-    def _bn(self, prefix, z, M, C, conv=None):
+    def _bn(self, prefix, z, M, C, conv):
+        """BatchNorm of the output z of `conv`, a unit added with stats=True"""
         b = Unit(prefix)
         b.prefix, b.z, b.M, b.C = prefix, z, M, C
-        b.partials, b.partial_rows = (conv.stats, conv.stats_rows) if conv is not None and conv.stats is not None else (None, 0)
+        b.partials, b.partial_rows = conv.stats, conv.stats_rows
         b.sums = self._buf(20 * C, dtype=torch.float64)  # 8 accumulator slots x {sum0, sum1} x C, arrival counter, backward coefficients
         b.mean, b.invstd, b.scale, b.shift = (self._buf(C, dtype=torch.float32) for _ in range(4))
         return b
@@ -559,71 +579,42 @@ class UNetTrainEngine:
                 if self._unpack_all is None:
                     self._grad(self.unpack_list[0][2])
                     self._unpack_all = []
-                    deterministic = os.environ.get("RSB_WGRAD_DETERMINISTIC", "1") != "0"
                     for ci, (chunk, used) in enumerate(self._dw_chunks):
                         gmap = torch.full((used, 4), -1, dtype=torch.int32, device=self.device)
                         for dwp, m, wname, c, off in self.unpack_list:
                             if c == ci:
                                 gmap[off:off + m.shape[0]] = torch.where(m >= 0, m + self._grad_offset[wname], m)
-                        if deterministic:
-                            # invert the scatter map once: every OIHW gradient element gathers its <= 4 packed contributions in order
-                            flat = gmap.reshape(-1).long()
-                            valid = flat >= 0
-                            src = flat[valid]
-                            pk = (torch.arange(flat.numel(), device=self.device) // 4)[valid]
-                            order = torch.argsort(src, stable=True)
-                            src, pk = src[order], pk[order]
-                            uniq, counts = torch.unique_consecutive(src, return_counts=True)
-                            assert int(counts.max()) <= 4, "a weight receives more than 4 packed gradient contributions"
-                            start = torch.cumsum(counts, 0) - counts
-                            gid = torch.repeat_interleave(torch.arange(uniq.numel(), device=self.device), counts)
-                            rank = torch.arange(src.numel(), device=self.device) - start[gid]
-                            inv = torch.full((uniq.numel(), 4), -1, dtype=torch.int32, device=self.device)
-                            inv[gid, rank] = pk.int()
-                            self._unpack_all.append(("gather", uniq.int().contiguous(), inv.contiguous(), chunk))
-                            del gmap
-                        else:
-                            self._unpack_all.append(("scatter", gmap, None, chunk, used))
-                for item in self._unpack_all:
-                    if item[0] == "gather":
-                        _, dst_idx, inv, chunk = item
-                        _lib.check(lib.rsb_unpack_grads_gather(chunk.data_ptr(), dst_idx.data_ptr(), inv.data_ptr(), self._grads_flat.data_ptr(),
-                                                               dst_idx.numel(), 1.0 / self.loss_scale, st), "rsb_unpack_grads_gather")
-                    else:
-                        _, gmap, _, chunk, used = item
-                        _lib.check(lib.rsb_unpack_grads(chunk.data_ptr(), gmap.data_ptr(), self._grads_flat.data_ptr(), used, 1.0 / self.loss_scale, st), "rsb_unpack_grads")
+                        self._unpack_all.append(invert_unpack_map(gmap) + (chunk,))
+                for dst_idx, inv, chunk in self._unpack_all:
+                    _lib.check(lib.rsb_unpack_grads_gather(chunk.data_ptr(), dst_idx.data_ptr(), inv.data_ptr(), self._grads_flat.data_ptr(),
+                                                           dst_idx.numel(), 1.0 / self.loss_scale, st), "rsb_unpack_grads_gather")
             elif k == "bn_stats":
-                # batch sums + (in the reduction's last block) statistics, folded scale/shift and the running-stat update
+                # batch statistics from the conv's partial sums: folded scale/shift and the running-stat update in the last block
                 b = op[1]
                 pf = b.prefix
-                if b.partials is not None:
-                    _lib.check(lib.rsb_bn_partials_finalize(b.partials.data_ptr(), b.partial_rows, b.sums.data_ptr(), P[pf + ".weight"].data_ptr(),
-                                                            P[pf + ".bias"].data_ptr(), P[pf + ".running_mean"].data_ptr(),
-                                                            P[pf + ".running_var"].data_ptr(), P[pf + ".num_batches_tracked"].data_ptr(),
-                                                            b.mean.data_ptr(), b.invstd.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), b.M, b.C,
-                                                            BN_EPS, BN_MOMENTUM, 1 if BN_CHAINED else 0, st), "rsb_bn_partials_finalize")
-                    continue
-                _lib.check((lib.rsb_bn_stats_finalize_chained if BN_CHAINED else lib.rsb_bn_stats_finalize)(b.z.data_ptr(), b.sums.data_ptr(), P[pf + ".weight"].data_ptr(), P[pf + ".bias"].data_ptr(),
-                                                     P[pf + ".running_mean"].data_ptr(), P[pf + ".running_var"].data_ptr(),
-                                                     P[pf + ".num_batches_tracked"].data_ptr(), b.mean.data_ptr(), b.invstd.data_ptr(),
-                                                     b.scale.data_ptr(), b.shift.data_ptr(), b.M, b.C, BN_EPS, BN_MOMENTUM, st), "rsb_bn_stats_finalize_chained")
+                assert b.partials is not None, pf
+                _lib.check(lib.rsb_bn_partials_finalize(b.partials.data_ptr(), b.partial_rows, b.sums.data_ptr(), P[pf + ".weight"].data_ptr(),
+                                                        P[pf + ".bias"].data_ptr(), P[pf + ".running_mean"].data_ptr(),
+                                                        P[pf + ".running_var"].data_ptr(), P[pf + ".num_batches_tracked"].data_ptr(),
+                                                        b.mean.data_ptr(), b.invstd.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), b.M, b.C,
+                                                        BN_EPS, BN_MOMENTUM, st), "rsb_bn_partials_finalize")
             elif k == "bn_finalize":
                 pass  # fused into the bn_stats launch (kept as an op for the CPU emulation of the plan)
             elif k == "bn_apply":
                 _, b, res, y, relu = op
-                _lib.check((lib.rsb_bn_apply_chained if BN_CHAINED else lib.rsb_bn_apply)(b.z.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), res.data_ptr() if res is not None else None,
-                                            y.data_ptr(), b.M, b.C, 1 if relu else 0, st), "rsb_bn_apply")
+                _lib.check(lib.rsb_bn_apply_chained(b.z.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), res.data_ptr() if res is not None else None,
+                                                    y.data_ptr(), b.M, b.C, 1 if relu else 0, st), "rsb_bn_apply_chained")
             elif k == "bn_bwd":
                 _, b, dy, y, dz, g = op
                 pf = b.prefix
                 # y = half(relu(z*scale + shift)) with no identity branch: the mask is re-derived from z, y is not read
                 zmask = y is not None and getattr(b, "plain_relu_y", None) is y
-                _lib.check((lib.rsb_bn_backward_chained if BN_CHAINED else lib.rsb_bn_backward)(dy.data_ptr(), y.data_ptr() if (y is not None and not zmask) else None, b.z.data_ptr(),
-                                               b.mean.data_ptr(), b.invstd.data_ptr(), P[pf + ".weight"].data_ptr(),
-                                               b.scale.data_ptr() if zmask else None, b.shift.data_ptr() if zmask else None,
-                                               b.sums.data_ptr(), dz.data_ptr(), g.data_ptr() if g is not None else None,
-                                               self._grad(pf + ".weight").data_ptr(), self._grad(pf + ".bias").data_ptr(), 1.0 / self.loss_scale,
-                                               b.M, b.C, st), "rsb_bn_backward")
+                _lib.check(lib.rsb_bn_backward_chained(dy.data_ptr(), y.data_ptr() if (y is not None and not zmask) else None, b.z.data_ptr(),
+                                                       b.mean.data_ptr(), b.invstd.data_ptr(), P[pf + ".weight"].data_ptr(),
+                                                       b.scale.data_ptr() if zmask else None, b.shift.data_ptr() if zmask else None,
+                                                       b.sums.data_ptr(), dz.data_ptr(), g.data_ptr() if g is not None else None,
+                                                       self._grad(pf + ".weight").data_ptr(), self._grad(pf + ".bias").data_ptr(), 1.0 / self.loss_scale,
+                                                       b.M, b.C, st), "rsb_bn_backward_chained")
             elif k == "relu_bwd":
                 _, a, b2, y, out = op
                 _lib.check(lib.rsb_relu_backward(a.data_ptr(), b2.data_ptr() if b2 is not None else None, y.data_ptr() if y is not None else None,

@@ -2,7 +2,7 @@
 # compute-sanitizer over one small convolution per kernel variant (fast, strict 3-MMA pair, strict N-concatenated, K-chunked) and
 # one weight-gradient case. The logs go to $OUT/sanitizer_*.log (default /tmp/rsb_sanitize).
 SAN=/usr/local/cuda/bin/compute-sanitizer
-SEL='test_conv_case_matches_cpu_reference[3] or test_conv_cta_pair_matches_single_cta[1] or test_split_conv_case_matches_fp64_reference[0] or test_split_conv_case_matches_fp64_reference[5] or test_split_conv_case_matches_fp64_reference[15] or test_wgrad_matches_cpu_emulation[2]'
+SEL='test_conv_case_matches_cpu_reference[3] or test_conv_cta_pair_matches_single_cta[1] or test_split_conv_case_matches_fp64_reference[0] or test_split_conv_case_matches_fp64_reference[5] or test_split_conv_case_matches_fp64_reference[15] or test_wgrad_split_k_scratch_matches_cpu_emulation[2]'
 OUT=${OUT:-/tmp/rsb_sanitize}
 mkdir -p "$OUT"
 for TOOL in memcheck synccheck racecheck; do

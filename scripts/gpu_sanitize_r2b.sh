@@ -2,7 +2,7 @@
 # compute-sanitizer over the kernels added late in round 2: the STATS epilogue of conv_tc_kernel (32/64-column chunks, 8 epilogue
 # warps, CTA pair), partial_reduce_kernel, pack_gather1_kernel (logs -> $OUT, default /tmp/rsb_sanitize).
 SAN=/usr/local/cuda/bin/compute-sanitizer
-SEL='test_conv_stats_epilogue_and_partials_finalize or test_relu_maxpool_final_pack_kernels'
+SEL='test_conv_stats_epilogue_partials_fold_to_float64_batchnorm or test_relu_maxpool_final_pack_unpack_kernels'
 OUT=${OUT:-/tmp/rsb_sanitize}
 mkdir -p "$OUT"
 for TOOL in memcheck synccheck; do

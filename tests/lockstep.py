@@ -14,7 +14,7 @@ Buffers pair by position (`_keep`, then the parameters, then the flat gradient b
      next op starts from identical inputs on both sides and a ReLU mask or max-pool argmax can never differ between them.
 
 Not compared (per-op scratch whose layout is the executor's business): BatchNorm accumulators `Unit.sums` (except that
-chained kernels must leave their slots and arrival counter zero), the conv-statistics partials (their column sums are
+the BatchNorm ops must leave their slots and arrival counter zero), the conv-statistics partials (their column sums are
 checked against the convolution's own output instead), `final_acc`, and the int32 weight-packing maps (constants).
 
 Tolerances, elementwise. u = 2^-24 is the fp32 unit roundoff; a tensor-core adder is not guaranteed to round to nearest,
@@ -84,10 +84,9 @@ def _f64(t):
 
 
 class EmulatorExecutor:
-    """Runs ops with the CPU emulator on a plan_only engine. Its BatchNorm ops clear their accumulators like the chained
-    kernels, and it is deterministic, but running a weight gradient twice would only repeat the same numpy call."""
+    """Runs ops with the CPU emulator on a plan_only engine. Its BatchNorm ops clear their accumulators like the kernels,
+    and it is deterministic, but running a weight gradient twice would only repeat the same numpy call."""
 
-    chained_bn = True
     repeat_wgrad = False
     conv_stats = False  # the emulated convolution does not write the BatchNorm partials (its bn_stats reads z)
 
@@ -111,10 +110,11 @@ class EmulatorExecutor:
 class GpuExecutor:
     """Runs ops kernel by kernel through UNetTrainEngine._run (graph replay is checked bit-identical elsewhere)."""
 
+    repeat_wgrad = True  # the split-K weight gradient must give the same bits when run twice
     conv_stats = True
 
-    def __init__(self, eng, chained_bn, repeat_wgrad):
-        self.eng, self.chained_bn, self.repeat_wgrad = eng, chained_bn, repeat_wgrad
+    def __init__(self, eng):
+        self.eng = eng
 
     def run(self, op, x=None, dlogits=None):
         self.eng._run([op], x=x, dlogits=dlogits)
@@ -405,7 +405,7 @@ class Lockstep(Harness):
                         c = int(np.argmax(err / tol))
                         self._fail(which, i, ot, u.name + ".stats", "%s of channel %d: partials give %r, float64 %r" % (
                             ("column sum", "sum of squares")[j], c, float(part[j][c]), float(ref[c])))
-        if k in ("bn_stats", "bn_bwd") and self.dut.chained_bn:
+        if k in ("bn_stats", "bn_bwd"):
             b = ot[1]
             idx, _ = self._locate(b.sums.data_ptr())
             acc = self.db[idx][:16 * b.C + 1]

@@ -228,10 +228,10 @@ def test_row_split_case_matches_fp64_reference(i, cuda_device):
     ("3x3", 4, 16, 16, 128, 256, 128, 1),   # CTA pair
     ("1x1", 3, 24, 16, 256, 512, 256, 1),   # CTA pair, odd number of spatial tiles (last pair half empty)
 ])
-def test_conv_stats_epilogue_and_partials_finalize(kind, N, H, W, cin, cout, block_n, pair, cuda_device):
-    """rsb_conv_desc.stats: the per-quarter-tile column sums of the fp16 outputs, written by the conv epilogue, fold to exactly
-    the BatchNorm batch statistics a reduction over the stored z gives (rsb_bn_stats_finalize): same mean / invstd / scale /
-    shift / running statistics to fp32 rounding; the conv output itself is bit-identical to the plain instance."""
+def test_conv_stats_epilogue_partials_fold_to_float64_batchnorm(kind, N, H, W, cin, cout, block_n, pair, cuda_device):
+    """rsb_conv_desc.stats: the per-quarter-tile column sums of the fp16 outputs, written by the conv epilogue, fold to the
+    float64 BatchNorm batch statistics of the stored z: same mean / invstd / scale / shift / running statistics to fp32
+    rounding; the conv output itself is bit-identical to the plain instance."""
     lib = _lib.load()
     stream = _lib.current_stream_ptr()
     case = conv_cases.conv_case(kind, N, H, W, cin, cout, cuda_device, seed=11, relu=False, bias=False, block_n=block_n, cta_pair=bool(pair))
@@ -259,30 +259,31 @@ def test_conv_stats_epilogue_and_partials_finalize(kind, N, H, W, cin, cout, blo
         assert torch.allclose(tot[0], z.sum(0), rtol=1e-5, atol=1e-3)
         assert torch.allclose(tot[1], (z * z).sum(0), rtol=1e-5, atol=1e-3)
 
-        def bn_buffers():
-            g = torch.Generator().manual_seed(3)
-            gamma = (torch.rand(cout, generator=g) + 0.5).to(cuda_device)
-            beta = torch.randn(cout, generator=g).to(cuda_device)
-            rm, rv = torch.zeros(cout, device=cuda_device), torch.ones(cout, device=cuda_device)
-            nb = torch.zeros(1, dtype=torch.int64, device=cuda_device)
-            outs = [torch.empty(cout, device=cuda_device) for _ in range(4)]
-            sums = torch.zeros(20 * cout, dtype=torch.float64, device=cuda_device)
-            return gamma, beta, rm, rv, nb, outs, sums
-
-        ga, be, rm, rv, nb, o1, sums = bn_buffers()
-        for chained in (1, 1, 0):  # chained twice: the accumulators are left clean for the next call
+        g = torch.Generator().manual_seed(3)
+        ga = (torch.rand(cout, generator=g) + 0.5).to(cuda_device)
+        be = torch.randn(cout, generator=g).to(cuda_device)
+        rm, rv = torch.zeros(cout, device=cuda_device), torch.ones(cout, device=cuda_device)
+        nb = torch.zeros(1, dtype=torch.int64, device=cuda_device)
+        o1 = [torch.empty(cout, device=cuda_device) for _ in range(4)]
+        sums = torch.zeros(20 * cout, dtype=torch.float64, device=cuda_device)
+        for _ in range(3):  # the accumulators are left clean for the next call
             _lib.check(lib.rsb_bn_partials_finalize(partials.data_ptr(), rows, sums.data_ptr(), ga.data_ptr(), be.data_ptr(), rm.data_ptr(),
-                                                    rv.data_ptr(), nb.data_ptr(), *[t.data_ptr() for t in o1], M, cout, 1e-5, 0.1, chained,
-                                                    stream), "partials_finalize")
-        ga2, be2, rm2, rv2, nb2, o2, sums2 = bn_buffers()
-        for _ in range(3):
-            _lib.check(lib.rsb_bn_stats_finalize(case.out.data_ptr(), sums2.data_ptr(), ga2.data_ptr(), be2.data_ptr(), rm2.data_ptr(),
-                                                 rv2.data_ptr(), nb2.data_ptr(), *[t.data_ptr() for t in o2], M, cout, 1e-5, 0.1, stream),
-                       "stats_finalize")
+                                                    rv.data_ptr(), nb.data_ptr(), *[t.data_ptr() for t in o1], M, cout, 1e-5, 0.1, stream),
+                       "partials_finalize")
         torch.cuda.synchronize()
-        assert int(nb) == 3 and int(nb2) == 3
-        for a, b in zip(o1 + [rm, rv], o2 + [rm2, rv2]):
-            assert torch.allclose(a, b, rtol=2e-5, atol=2e-6), (a - b).abs().max()
+        assert int(nb) == 3
+        # float64 reference: biased variance for the normalisation, the unbiased one for the running update (momentum 0.1)
+        mean = z.sum(0) / M
+        var = ((z * z).sum(0) / M - mean * mean).clamp_min(0)
+        invstd = 1.0 / torch.sqrt(var + 1e-5)
+        scale = ga.double() * invstd
+        shift = be.double() - mean * scale
+        rm_ref, rv_ref = torch.zeros_like(mean), torch.ones_like(mean)
+        for _ in range(3):
+            rm_ref = 0.9 * rm_ref + 0.1 * mean
+            rv_ref = 0.9 * rv_ref + 0.1 * var * M / (M - 1)
+        for got, want in zip(o1 + [rm, rv], [mean, invstd, scale, shift, rm_ref, rv_ref]):
+            assert torch.allclose(got.double(), want, rtol=2e-5, atol=2e-6), (got.double() - want).abs().max()
     finally:
         lib.rsb_conv_plan_destroy(plan)
 

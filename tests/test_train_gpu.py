@@ -27,7 +27,7 @@ def _rel(a, b):
     return ((a - b).pow(2).sum().sqrt() / b.pow(2).sum().sqrt().clamp_min(1e-30)).item()
 
 
-def test_batchnorm_train_kernels(cuda_device):
+def test_batchnorm_chained_train_kernels(cuda_device):
     lib, st = _lib.load(), _lib.current_stream_ptr()
     g = torch.Generator().manual_seed(0)
     for (M, C) in [(2 * 16 * 16, 64), (3 * 8 * 8, 2048), (5 * 7 * 9, 256), (4 * 96 * 96, 128)]:  # last: > 1000 blocks
@@ -46,17 +46,24 @@ def test_batchnorm_train_kernels(cuda_device):
         zd, resd, dyd = z.to(d), res.to(d), dy.to(d)
         gd, bd, rmd, rvd = gamma.to(d), beta.to(d), rm.to(d), rv.to(d)
         nb = torch.zeros((), dtype=torch.int64, device=d)
-        sums = torch.zeros(20 * C, dtype=torch.float64, device=d)
+        sums = torch.zeros(20 * C, dtype=torch.float64, device=d)  # zeroed once: every kernel below leaves it zeroed again
         mean, invstd, scale, shift = (torch.zeros(C, device=d) for _ in range(4))
         y = torch.zeros((M, C), dtype=torch.float16, device=d)
-        _lib.check(lib.rsb_bn_stats(zd.data_ptr(), sums.data_ptr(), M, C, st), "stats")
-        _lib.check(lib.rsb_bn_finalize(sums.data_ptr(), gd.data_ptr(), bd.data_ptr(), rmd.data_ptr(), rvd.data_ptr(), nb.data_ptr(), mean.data_ptr(),
-                                       invstd.data_ptr(), scale.data_ptr(), shift.data_ptr(), C, M, 1e-5, 0.1, st), "finalize")
-        _lib.check(lib.rsb_bn_apply(zd.data_ptr(), scale.data_ptr(), shift.data_ptr(), resd.data_ptr(), y.data_ptr(), M, C, 1, st), "apply")
+        # the statistics input a convolution epilogue writes: [rows][2][C] fp32 column sums / sums of squares of 32-row blocks
+        rows = -(-M // 32)
+        zb = torch.zeros((rows * 32, C), dtype=torch.float64)
+        zb[:M] = z.double()
+        zb = zb.reshape(rows, 32, C)
+        partials = torch.stack((zb.sum(1), (zb * zb).sum(1)), 1).float().contiguous().to(d)
+        _lib.check(lib.rsb_bn_partials_finalize(partials.data_ptr(), rows, sums.data_ptr(), gd.data_ptr(), bd.data_ptr(), rmd.data_ptr(),
+                                                rvd.data_ptr(), nb.data_ptr(), mean.data_ptr(), invstd.data_ptr(), scale.data_ptr(),
+                                                shift.data_ptr(), M, C, 1e-5, 0.1, st), "partials_finalize")
+        _lib.check(lib.rsb_bn_apply_chained(zd.data_ptr(), scale.data_ptr(), shift.data_ptr(), resd.data_ptr(), y.data_ptr(), M, C, 1, st), "apply")
         dz, gout = torch.zeros_like(y), torch.zeros_like(y)
         dg, db = torch.zeros(C, device=d), torch.zeros(C, device=d)
-        _lib.check(lib.rsb_bn_backward(dyd.data_ptr(), y.data_ptr(), zd.data_ptr(), mean.data_ptr(), invstd.data_ptr(), gd.data_ptr(), None, None,
-                                       sums.data_ptr(), dz.data_ptr(), gout.data_ptr(), dg.data_ptr(), db.data_ptr(), 0.5, M, C, st), "bwd")
+        _lib.check(lib.rsb_bn_backward_chained(dyd.data_ptr(), y.data_ptr(), zd.data_ptr(), mean.data_ptr(), invstd.data_ptr(), gd.data_ptr(), None,
+                                               None, sums.data_ptr(), dz.data_ptr(), gout.data_ptr(), dg.data_ptr(), db.data_ptr(), 0.5, M, C, st),
+                   "bwd")
         torch.cuda.synchronize()
         yr = y_ref.detach().reshape(C, M).t()
         assert (y.float().cpu() - yr).abs().max().item() <= 4e-3 * max(1.0, yr.abs().max().item() / 4)
@@ -67,33 +74,22 @@ def test_batchnorm_train_kernels(cuda_device):
         assert _rel(gout.float().cpu(), dy.float() * mask) < 1e-3
         # plain relu(bn(z)) (no identity branch): the mask re-derived from z gives the same bits as the mask read from y
         y2 = torch.zeros_like(y)
-        _lib.check(lib.rsb_bn_apply(zd.data_ptr(), scale.data_ptr(), shift.data_ptr(), None, y2.data_ptr(), M, C, 1, st), "apply")
+        _lib.check(lib.rsb_bn_apply_chained(zd.data_ptr(), scale.data_ptr(), shift.data_ptr(), None, y2.data_ptr(), M, C, 1, st), "apply")
         outs = []
         for use_z in (False, True):
             dz2, go2 = torch.zeros_like(y), torch.zeros_like(y)
             dg2, db2 = torch.zeros(C, device=d), torch.zeros(C, device=d)
-            _lib.check(lib.rsb_bn_backward(dyd.data_ptr(), None if use_z else y2.data_ptr(), zd.data_ptr(), mean.data_ptr(), invstd.data_ptr(), gd.data_ptr(),
-                                           scale.data_ptr() if use_z else None, shift.data_ptr() if use_z else None, sums.data_ptr(), dz2.data_ptr(),
-                                           go2.data_ptr(), dg2.data_ptr(), db2.data_ptr(), 1.0, M, C, st), "bwd")
+            _lib.check(lib.rsb_bn_backward_chained(dyd.data_ptr(), None if use_z else y2.data_ptr(), zd.data_ptr(), mean.data_ptr(), invstd.data_ptr(),
+                                                   gd.data_ptr(), scale.data_ptr() if use_z else None, shift.data_ptr() if use_z else None,
+                                                   sums.data_ptr(), dz2.data_ptr(), go2.data_ptr(), dg2.data_ptr(), db2.data_ptr(), 1.0, M, C, st), "bwd")
             torch.cuda.synchronize()
             outs.append((dz2.clone(), go2.clone(), dg2.clone(), db2.clone()))
         assert torch.equal(outs[0][1], outs[1][1])  # the masked gradient: identical masks
         assert torch.allclose(outs[0][0].float(), outs[1][0].float(), atol=2e-3, rtol=2e-3)  # dz: fp64 atomics may reorder the sums' last bits
         assert torch.allclose(outs[0][2], outs[1][2], rtol=1e-5, atol=1e-6) and torch.allclose(outs[0][3], outs[1][3], rtol=1e-5, atol=1e-6)
-        # one-launch variant used by the engine: statistics + finalize in the reduction's last block
-        rm2, rv2 = rm.to(d), rv.to(d)
-        nb2 = torch.zeros((), dtype=torch.int64, device=d)
-        outs2 = [torch.zeros(C, device=d) for _ in range(4)]
-        _lib.check(lib.rsb_bn_stats_finalize(zd.data_ptr(), sums.data_ptr(), gd.data_ptr(), bd.data_ptr(), rm2.data_ptr(), rv2.data_ptr(), nb2.data_ptr(),
-                                             outs2[0].data_ptr(), outs2[1].data_ptr(), outs2[2].data_ptr(), outs2[3].data_ptr(), M, C, 1e-5, 0.1, st),
-                   "stats_finalize")
-        torch.cuda.synchronize()
-        for got, want in zip(outs2 + [rm2, rv2], [mean, invstd, scale, shift, rmd, rvd]):
-            assert torch.allclose(got, want, rtol=1e-6, atol=1e-6)
-        assert int(nb2.item()) == 1
 
 
-def test_relu_maxpool_final_pack_kernels(cuda_device):
+def test_relu_maxpool_final_pack_unpack_kernels(cuda_device):
     lib, st, d = _lib.load(), _lib.current_stream_ptr(), cuda_device
     g = torch.Generator().manual_seed(1)
     # relu backward with fan-in
@@ -144,7 +140,7 @@ def test_relu_maxpool_final_pack_kernels(cuda_device):
     assert _rel(dy5.float().cpu() / 256.0, y5t.grad.permute(0, 2, 3, 1)) < 2e-3
     assert _rel(dw.cpu(), w.grad) < 1e-4 and _rel(dbv.cpu(), bb.grad) < 1e-5
     # pack / unpack with the upsample-phase map (sums of up to 4 taps)
-    from robosat_b200.train_engine import map_up_fwd
+    from robosat_b200.train_engine import invert_unpack_map, map_up_fwd
     from robosat_b200.engine import pack_upsample_phases
 
     wt = torch.randn((8, 64, 3, 3), generator=g)
@@ -157,7 +153,8 @@ def test_relu_maxpool_final_pack_kernels(cuda_device):
     gp = torch.randn(m.shape[0], generator=g)
     grad = torch.zeros_like(wt).to(d)
     gpd = gp.to(d)
-    _lib.check(lib.rsb_unpack_grads(gpd.data_ptr(), m.data_ptr(), grad.data_ptr(), m.shape[0], 0.5, st), "unpack")
+    dst_idx, inv4 = invert_unpack_map(m)
+    _lib.check(lib.rsb_unpack_grads_gather(gpd.data_ptr(), dst_idx.data_ptr(), inv4.data_ptr(), grad.data_ptr(), dst_idx.numel(), 0.5, st), "unpack")
     torch.cuda.synchronize()
     wref = wt.clone().requires_grad_(True)
     (pack_upsample_phases(wref).reshape(-1) * gp * 0.5).sum().backward()
@@ -179,7 +176,7 @@ def test_relu_maxpool_final_pack_kernels(cuda_device):
 
 
 @pytest.mark.parametrize("i", range(len(conv_cases.default_cases(None)) - 2))  # head cases have no packed fp16 output
-def test_wgrad_matches_cpu_emulation(i, cuda_device):
+def test_wgrad_split_k_scratch_matches_cpu_emulation(i, cuda_device):
     lib, st = _lib.load(), _lib.current_stream_ptr()
     case = conv_cases.default_cases(cuda_device)[i]()
     cpu = conv_cases.default_cases("cpu")[i]()
@@ -191,7 +188,10 @@ def test_wgrad_matches_cpu_emulation(i, cuda_device):
     dyd = dy.to(cuda_device)
     plan = ctypes.c_void_p()
     _lib.check(lib.rsb_wgrad_plan_create(ctypes.byref(d), dyd.data_ptr(), dw.data_ptr(), ctypes.byref(plan)), "wgrad_plan")
-    for _ in range(2):
+    need = int(lib.rsb_wgrad_plan_scratch_bytes(plan))  # split-K plans keep their per-slice partials there
+    scratch = torch.empty(need // 4 + 4, dtype=torch.float32, device=cuda_device)
+    _lib.check(lib.rsb_wgrad_plan_set_scratch(plan, scratch.data_ptr(), need), "wgrad_set_scratch")
+    for _ in range(2):  # the second run overwrites dw, it does not add to it
         _lib.check(lib.rsb_wgrad_run(plan, st), "wgrad_run")
     torch.cuda.synchronize()
     ref = torch.zeros(d.phases * d.Cout * K, dtype=torch.float32)
@@ -480,7 +480,7 @@ def test_backward_is_deterministic(cuda_device):
         grads = eng.backward(dlogits)
         torch.cuda.synchronize()
         runs.append({k: v.clone() for k, v in grads.items()})
-    assert getattr(eng, "_wgrad_scratch", None) is not None, "no wgrad plan needed a scratch: the test would be vacuous"
+    assert eng._wgrad_scratch is not None, "no wgrad plan needed a scratch: the test would be vacuous"
     for k in runs[0]:
         assert torch.equal(runs[0][k], runs[1][k]), k
 

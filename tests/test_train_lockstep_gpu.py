@@ -20,7 +20,7 @@ pytestmark = pytest.mark.gpu
 # --------------------------------------------------------------------------------------------------
 # the whole training step in lockstep
 # --------------------------------------------------------------------------------------------------
-def _lockstep(cuda_device, C, B, H, W, dlogits_from_ce, chained=True, deterministic=True):
+def _lockstep(cuda_device, C, B, H, W, dlogits_from_ce):
     _, dut, twin = lockstep.make_pair(C, B, H, W, 1024.0, cuda_device)
     x = synth.normalize_tiles(synth.make_tiles_u8(B, max(H, W), seed=1))[:, :, :H, :W].contiguous()
     if dlogits_from_ce:
@@ -39,7 +39,7 @@ def _lockstep(cuda_device, C, B, H, W, dlogits_from_ce, chained=True, determinis
         dlogits = dl.cpu()
     else:
         dlogits = torch.randn((B, C, H, W), generator=torch.Generator().manual_seed(3)) * 1e-3
-    ex = lockstep.GpuExecutor(dut, chained_bn=chained, repeat_wgrad=deterministic)
+    ex = lockstep.GpuExecutor(dut)
     ls = lockstep.Lockstep(ex, twin)
     ls.run(x, dlogits, dut_x=x.to(cuda_device), dut_dlogits=dlogits.to(cuda_device))
     print("\n%d x %d x %d x %d, %d classes:\n%s" % (B, 3, H, W, C, ls.table()))
@@ -51,7 +51,7 @@ def test_train_step_lockstep_128(cuda_device):
     dut, ls = _lockstep(cuda_device, 2, 2, 128, 128, dlogits_from_ce=True)
     assert lockstep.n_ops(dut) == 413
     lib = _lib.load()
-    plans = dut.__dict__.get("_wgrad_plans", [])
+    plans = dut._wgrad_plans
     assert len(plans) == 60 and any(lib.rsb_wgrad_plan_scratch_bytes(p) > 0 for p in plans), \
         "no weight-gradient plan used the deterministic split-K scratch: its reduction would be unchecked"
 
@@ -60,17 +60,8 @@ def test_train_step_lockstep_rectangular_six_classes(cuda_device):
     _lockstep(cuda_device, 6, 3, 64, 128, dlogits_from_ce=False)
 
 
-def test_train_step_lockstep_unchained_paths(cuda_device, monkeypatch):
-    """the non-default paths: BatchNorm statistics re-read z, separate (memset) BatchNorm launches, fp32-atomic split-K"""
-    monkeypatch.setattr(train_engine, "CONV_STATS", False)
-    monkeypatch.setattr(train_engine, "BN_CHAINED", False)
-    monkeypatch.setenv("RSB_WGRAD_DETERMINISTIC", "0")
-    dut, _ = _lockstep(cuda_device, 2, 2, 64, 64, dlogits_from_ce=False, chained=False, deterministic=False)
-    assert all(u.stats is None for u in dut.units.values()) and dut.__dict__.get("_wgrad_scratch") is None
-
-
 # --------------------------------------------------------------------------------------------------
-# weight gradients: split-K with and without the deterministic scratch, ragged tilings
+# weight gradients: split-K through the scratch (own and shared), a missing scratch refused, ragged tilings
 # --------------------------------------------------------------------------------------------------
 def _wgrad_cases(dev):
     """(name, desc, dy tensor, dy element offset, keep-alive) for engine layers and synthetic ragged shapes"""
@@ -128,7 +119,7 @@ def _check_wgrad(name, got, ref, tol):
     return worst
 
 
-def test_wgrad_split_k_paths_match_float64(cuda_device):
+def test_wgrad_split_k_matches_float64_and_needs_scratch(cuda_device):
     lib, st = _lib.load(), _lib.current_stream_ptr()
     cases = _wgrad_cases(cuda_device)
     refs, plans, outs = [], [], []
@@ -153,10 +144,11 @@ def test_wgrad_split_k_paths_match_float64(cuda_device):
     try:
         for (name, d, dy, off, keep), plan, dw, (ref, tol) in zip(cases, plans, outs, refs):
             need = int(lib.rsb_wgrad_plan_scratch_bytes(plan))
-            # 1. fp32-atomic split-K (no scratch)
-            _lib.check(lib.rsb_wgrad_run(plan, st), "wgrad_run")
+            # 1. no scratch yet: refused before any launch, dw left as it was
+            assert lib.rsb_wgrad_run(plan, st) != 0, name
+            assert "rsb_wgrad_plan_set_scratch" in _lib.last_error(), _lib.last_error()
             torch.cuda.synchronize()
-            worst[name + " atomics"] = _check_wgrad(name + " atomics", dw, ref, tol)
+            assert bool(torch.isnan(dw).all()), name
             # 2. deterministic split-K: twice, bit-identical
             scratch = torch.empty(need // 4 + 4, dtype=torch.float32, device=cuda_device)
             _lib.check(lib.rsb_wgrad_plan_set_scratch(plan, scratch.data_ptr(), need), "set_scratch")
