@@ -225,6 +225,12 @@ int rsb_augment_dihedral(const uint8_t* img, const uint8_t* mask, const int32_t*
  * logits fp32 [N][2][H][W] -> quant uint8 [N][H-2o][W-2o]; probs_fg (fp32, same cropped shape) optional. */
 int rsb_head_quantize(const float* logits, uint8_t* quant, float* probs_fg, int32_t N, int32_t H, int32_t W,
                       int32_t overlap, void* stream);
+/* Predict head for C = 2..255 classes (`rs predict` of a multi-class model; no reference counterpart): per pixel the softmax of
+ * rsb_head_tta_accumulate (max over the classes in order, class-ordered sum of expf(l - max), one division), the crop of `overlap`,
+ * then np.digitize(p, linspace(0, 1, 256)).astype(uint8) of EVERY class. logits fp32 [N][C][H][W] -> quant uint8
+ * [N][C][H-2o][W-2o]; probs (fp32, same shape) optional. For C = 2, plane 1 equals rsb_head_quantize's output bit for bit. */
+int rsb_head_quantize_classes(const float* logits, uint8_t* quant, float* probs, int32_t N, int32_t C, int32_t H, int32_t W,
+                              int32_t overlap, void* stream);
 /* softmax over C for any class count: logits fp32 [N][C][H][W] -> probs fp32 same shape (predict.py:87) */
 int rsb_softmax_nchw(const float* logits, float* probs, int32_t N, int32_t C, int32_t HW, void* stream);
 /* `buffer_tile_image` (robosat/tiles.py:162-227) on the device: builds B buffered tiles uint8 [B][S+2o][S+2o][3] from a cache of
@@ -234,6 +240,10 @@ int rsb_stitch_halo(const uint8_t* cache, const int32_t* slots, uint8_t* out, in
 /* `rs masks` soft vote (robosat/tools/masks.py:42-84): quant uint8 [K][n] probability bins of K models (as written by rs predict),
  * weights float64 [K] on the device or NULL -> mask uint8 [n] = argmax([1 - p, p]) of the weighted average, float64, numpy's order. */
 int rsb_softvote(const uint8_t* quant, const double* weights, uint8_t* mask, int32_t K, int64_t n, void* stream);
+/* `rs masks --dataset` for C = 2..255 classes: quant uint8 [K][C][n] (per model the C probability planes rs predict writes for a
+ * multi-class model), weights float64 [K] on the device or NULL -> mask uint8 [n] = np.argmax(np.average(anchors[quant], axis=0,
+ * weights=w), axis=0): float64, sequential sum over K, products and sums rounded separately, one division, first maximum wins. */
+int rsb_softvote_classes(const uint8_t* quant, const double* weights, uint8_t* mask, int32_t K, int32_t C, int64_t n, void* stream);
 /* `rs weights` histogram (robosat/tools/weights.py:39-49): counts[c] += #(labels == c) for c < C; counts is uint64 [C] on the device */
 int rsb_class_histogram(const uint8_t* labels, int64_t n, int32_t C, uint64_t* counts, void* stream);
 /* `Predictor.segment` head (robosat/tools/serve.py:150-165): output.argmax(axis=0).astype(uint8) of fp32 NCHW logits
@@ -253,6 +263,9 @@ int rsb_head_tta_accumulate(const float* logits, int64_t* acc, const int32_t* op
 /* 2-class acc [B][2][HW] summed over `views` views -> quant uint8 [B][HW]: np.digitize bins of the mean foreground probability
  * (float)(acc[b][1] * 2^-59 / views), as rsb_head_quantize bins a single view */
 int rsb_head_tta_quantize(const int64_t* acc, uint8_t* quant, int32_t B, int32_t HW, int32_t views, void* stream);
+/* acc int64 [B][C][HW] summed over `views` views -> quant uint8 [B][C][HW]: every class binned as rsb_head_tta_quantize bins
+ * class 1, (float)(acc * 2^-59 / views); C = 2..255 */
+int rsb_head_tta_quantize_classes(const int64_t* acc, uint8_t* quant, int32_t B, int32_t C, int32_t HW, int32_t views, void* stream);
 /* acc int64 [B][C][HW] -> uint8 [B][HW]: class of the largest sum (= largest mean probability), first maximum wins; C <= 255 */
 int rsb_head_tta_argmax(const int64_t* acc, uint8_t* mask, int32_t B, int32_t C, int32_t HW, void* stream);
 /* rsb_augment_dihedral's image transform for H x W tiles without a mask; when H != W only the flip bit of each op is used */

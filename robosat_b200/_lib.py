@@ -196,6 +196,9 @@ SIGNATURES = {
     "rsb_head_tta_accumulate": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(_i32), _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "rsb_head_tta_quantize": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_head_tta_argmax": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "rsb_head_quantize_classes": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "rsb_head_tta_quantize_classes": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "rsb_softvote_classes": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "rsb_augment_flip_rect": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_morph_binary": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, ctypes.POINTER(MorphOp), _i32, _vp, _vp, _vp]),
     "rsb_rasterize_polygons": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]),

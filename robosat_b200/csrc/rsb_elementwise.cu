@@ -405,6 +405,97 @@ __global__ void softvote_kernel(const uint8_t* __restrict__ quant, const double*
     }
 }
 
+// Softmax of one pixel over C classes, as torch.softmax and head_tta_accumulate_kernel compute it: m = fmaxf over the classes in
+// order, s = the class-ordered sum of expf(l_c - m); then p_c = expf(l_c - m) / s (`softmax_prob`). `l` points at class 0 of the
+// pixel, classes `cstride` floats apart. For C = 2 this is head_quantize_kernel's e1 / (e0 + e1) bit for bit (0 + e0 == e0).
+__device__ __forceinline__ void softmax_pixel(const float* __restrict__ l, int64_t cstride, int C, float& m, float& s) {
+    m = __ldg(l);
+    for (int c = 1; c < C; ++c) m = fmaxf(m, __ldg(l + c * cstride));
+    s = 0.f;
+    for (int c = 0; c < C; ++c) s += expf(__ldg(l + c * cstride) - m);
+}
+
+__device__ __forceinline__ float softmax_prob(float l, float m, float s) { return expf(l - m) / s; }
+
+// `rs predict` for C classes: softmax -> crop `o` -> np.digitize of every class plane. One thread per 4 adjacent pixels of a cropped
+// row: the three class-ordered passes re-read the thread's own logits (cache hits; HBM sees each logit once), and each plane's 4
+// bins go out as one 32-bit word when the cropped width is a multiple of 4 (`vec`), else as single bytes.
+__global__ void head_quantize_classes_kernel(const float* __restrict__ logits, uint8_t* __restrict__ quant, float* __restrict__ probs, int N,
+                                             int C, int H, int W, int o, int vec) {
+    const int OH = H - 2 * o, OW = W - 2 * o;
+    const int groups = (OW + 3) / 4;
+    const int64_t total = static_cast<int64_t>(N) * OH * groups;
+    const int64_t hw = static_cast<int64_t>(H) * W, ohw = static_cast<int64_t>(OH) * OW;
+    for (int64_t gid = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; gid < total; gid += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int x0 = static_cast<int>(gid % groups) * 4;
+        const int y = static_cast<int>((gid / groups) % OH);
+        const int n = static_cast<int>(gid / (static_cast<int64_t>(groups) * OH));
+        const int npx = min(4, OW - x0);
+        const float* l = logits + static_cast<int64_t>(n) * C * hw + static_cast<int64_t>(y + o) * W + (x0 + o);
+        float m[4], s[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (j < npx) softmax_pixel(l + j, hw, C, m[j], s[j]);
+        const int64_t out0 = static_cast<int64_t>(n) * C * ohw + static_cast<int64_t>(y) * OW + x0;
+        for (int c = 0; c < C; ++c) {
+            const int64_t out = out0 + c * ohw;
+            float p[4];
+            uint32_t word = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                p[j] = j < npx ? softmax_prob(__ldg(l + c * hw + j), m[j], s[j]) : 0.f;
+                word |= static_cast<uint32_t>(static_cast<uint8_t>(digitize256(p[j]))) << (8 * j);  // 256 wraps to 0 like .astype(np.uint8)
+            }
+            if (vec) {
+                *reinterpret_cast<uint32_t*>(quant + out) = word;
+                if (probs) *reinterpret_cast<float4*>(probs + out) = make_float4(p[0], p[1], p[2], p[3]);
+            } else {
+                for (int j = 0; j < npx; ++j) {
+                    quant[out + j] = static_cast<uint8_t>(word >> (8 * j));
+                    if (probs) probs[out + j] = p[j];
+                }
+            }
+        }
+    }
+}
+
+// every class of acc [N][C][HW] summed over `views` views -> np.digitize bins of (float)(acc * 2^-59 / views), as
+// head_tta_quantize_kernel bins class 1
+__global__ void head_tta_quantize_classes_kernel(const int64_t* __restrict__ acc, uint8_t* __restrict__ quant, int64_t total, int views) {
+    for (int64_t gid = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; gid < total; gid += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const float p = static_cast<float>(static_cast<double>(acc[gid]) * (1.0 / kTtaOne) / views);
+        quant[gid] = static_cast<uint8_t>(digitize256(p));
+    }
+}
+
+// `rs masks --dataset` for C classes: np.argmax(np.average(anchors[q], axis=0, weights=w), axis=0) over quant [K][C][n], float64 in
+// numpy's order like softvote_kernel: per class a sequential sum over the K models (products rounded on their own), one division by
+// the weight sum / K, then the first maximum. Dividing before comparing matters: it can round two different sums to one value.
+__global__ void softvote_classes_kernel(const uint8_t* __restrict__ quant, const double* __restrict__ weights, uint8_t* __restrict__ mask, int K,
+                                        int C, int64_t n) {
+    const double step = 1.0 / 255.0;
+    double scl = 0.0;
+    for (int k = 0; k < K; ++k) scl += weights ? weights[k] : 1.0;
+    for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        double best = 0.0;
+        int arg = 0;
+        for (int c = 0; c < C; ++c) {
+            double sum = 0.0;
+            for (int k = 0; k < K; ++k) {
+                const int q = quant[(static_cast<int64_t>(k) * C + c) * n + i];
+                const double p = q >= 255 ? 1.0 : static_cast<double>(q) * step;  // linspace pins its last anchor to 1.0
+                sum = weights ? __dadd_rn(sum, __dmul_rn(p, weights[k])) : sum + p;
+            }
+            const double avg = sum / scl;
+            if (c == 0 || avg > best) {
+                best = avg;
+                arg = c;
+            }
+        }
+        mask[i] = static_cast<uint8_t>(arg);
+    }
+}
+
 // `rs weights` (robosat/tools/weights.py:39-49): np.bincount of the training masks, per class, accumulated over calls
 __global__ void class_histogram_kernel(const uint8_t* __restrict__ labels, int64_t n, int C, unsigned long long* __restrict__ counts) {
     __shared__ unsigned int sh[256];
@@ -613,6 +704,36 @@ extern "C" int rsb_softvote(const uint8_t* quant, const double* weights, uint8_t
     softvote_kernel<<<grid_for(n, 256) > 132 * 16 ? 132 * 16 : grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(quant, weights, mask, K, n);
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "softvote launch");
+}
+
+extern "C" int rsb_head_quantize_classes(const float* logits, uint8_t* quant, float* probs, int32_t N, int32_t C, int32_t H, int32_t W,
+                                         int32_t overlap, void* stream) {
+    if (!logits || !quant || N <= 0 || C < 2 || C > 255 || overlap < 0 || H - 2 * overlap <= 0 || W - 2 * overlap <= 0)
+        return set_error(RSB_E_INVALID, "head_quantize_classes: bad arguments (C must be 2..255, 2*overlap < H and W)");
+    const int OH = H - 2 * overlap, OW = W - 2 * overlap;
+    const int vec = OW % 4 == 0 && (reinterpret_cast<uintptr_t>(quant) & 3) == 0 && (reinterpret_cast<uintptr_t>(probs) & 15) == 0;
+    const int64_t total = static_cast<int64_t>(N) * OH * ((OW + 3) / 4);
+    const unsigned blocks = grid_for(total, 256) > 132 * 32 ? 132 * 32 : grid_for(total, 256);
+    head_quantize_classes_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(logits, quant, probs, N, C, H, W, overlap, vec);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "head_quantize_classes launch");
+}
+
+extern "C" int rsb_head_tta_quantize_classes(const int64_t* acc, uint8_t* quant, int32_t B, int32_t C, int32_t HW, int32_t views, void* stream) {
+    if (!acc || !quant || B <= 0 || C < 2 || C > 255 || HW <= 0 || views < 1) return set_error(RSB_E_INVALID, "head_tta_quantize_classes: bad arguments");
+    const int64_t total = static_cast<int64_t>(B) * C * HW;
+    const unsigned blocks = grid_for(total, 256) > 132 * 32 ? 132 * 32 : grid_for(total, 256);
+    head_tta_quantize_classes_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(acc, quant, total, views);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "head_tta_quantize_classes launch");
+}
+
+extern "C" int rsb_softvote_classes(const uint8_t* quant, const double* weights, uint8_t* mask, int32_t K, int32_t C, int64_t n, void* stream) {
+    if (!quant || !mask || K < 1 || C < 2 || C > 255 || n <= 0) return set_error(RSB_E_INVALID, "softvote_classes: bad arguments");
+    softvote_classes_kernel<<<grid_for(n, 256) > 132 * 16 ? 132 * 16 : grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(quant, weights, mask,
+                                                                                                                                  K, C, n);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? RSB_OK : set_cuda_error(e, "softvote_classes launch");
 }
 
 extern "C" int rsb_class_histogram(const uint8_t* labels, int64_t n, int32_t C, uint64_t* counts, void* stream) {

@@ -35,13 +35,15 @@ class TilePredictor:
             self.tta = TtaChain(self.engine, tta, batch, size, size, num_classes, overlap, device=self.device)
         self.out_size = size - 2 * overlap
         self.depth = depth
+        # 2 classes: the foreground bins [B, h, w]; more: the bins of every class [B, C, h, w]
+        out_shape = (batch, self.out_size, self.out_size) if num_classes == 2 else (batch, num_classes, self.out_size, self.out_size)
         self._slots = []
         for _ in range(depth):
             self._slots.append({
                 "h_in": torch.empty((batch, size, size, 3), dtype=torch.uint8, pin_memory=True),
                 "d_in": torch.empty((batch, size, size, 3), dtype=torch.uint8, device=self.device),
-                "d_q": torch.empty((batch, self.out_size, self.out_size), dtype=torch.uint8, device=self.device),
-                "h_q": torch.empty((batch, self.out_size, self.out_size), dtype=torch.uint8, pin_memory=True),
+                "d_q": torch.empty(out_shape, dtype=torch.uint8, device=self.device),
+                "h_q": torch.empty(out_shape, dtype=torch.uint8, pin_memory=True),
                 "done": torch.cuda.Event(),
                 "loaded": torch.cuda.Event(),
                 "consumed": torch.cuda.Event(),
@@ -52,9 +54,9 @@ class TilePredictor:
         self._next = 0
         self._pending = []
         self.h2d_bytes = batch * size * size * 3
-        self.d2h_bytes = batch * self.out_size * self.out_size
+        self.d2h_bytes = batch * self.out_size * self.out_size * (1 if num_classes == 2 else num_classes)
         self.graph_error = None
-        if use_graph and num_classes == 2:
+        if use_graph and num_classes >= 2:
             self._capture_graphs()
 
     def _compute(self, slot):
@@ -99,11 +101,18 @@ class TilePredictor:
         return self.engine.forward(x_dev)
 
     def quantize(self, logits, out_u8, probs=None):
-        """softmax -> foreground -> crop overlap -> np.digitize bins (predict.py:87-103), binary models only."""
-        assert self.classes == 2, "single channel requires binary model"  # predict.py:98
+        """softmax -> crop overlap -> np.digitize bins (predict.py:87-103): of the foreground [B, h, w] for a binary model, of every
+        class [B, C, h, w] for C > 2 (`rsb_head_quantize_classes`). `probs` (optional, fp32, the shape of `out_u8`) receives the
+        probabilities that were binned."""
+        assert self.classes >= 2, "single channel requires binary model"  # predict.py:98
         lib = _lib.load()
-        _lib.check(lib.rsb_head_quantize(logits.data_ptr(), out_u8.data_ptr(), probs.data_ptr() if probs is not None else None,
-                                         self.batch, self.size, self.size, self.overlap, _lib.current_stream_ptr()), "rsb_head_quantize")
+        pp = probs.data_ptr() if probs is not None else None
+        if self.classes == 2:
+            _lib.check(lib.rsb_head_quantize(logits.data_ptr(), out_u8.data_ptr(), pp, self.batch, self.size, self.size, self.overlap,
+                                             _lib.current_stream_ptr()), "rsb_head_quantize")
+        else:
+            _lib.check(lib.rsb_head_quantize_classes(logits.data_ptr(), out_u8.data_ptr(), pp, self.batch, self.classes, self.size, self.size,
+                                                     self.overlap, _lib.current_stream_ptr()), "rsb_head_quantize_classes")
         return out_u8
 
     def num_launches(self):
@@ -113,7 +122,8 @@ class TilePredictor:
 
     # ------------------------------------------------------------------ host -> host
     def predict_u8(self, tiles_u8_host):
-        """Blocking: host uint8 [B, S, S, 3] -> host uint8 [B, S-2o, S-2o] quantised foreground probability."""
+        """Blocking: host uint8 [B, S, S, 3] -> host uint8 [B, S-2o, S-2o] quantised foreground probability ([B, C, S-2o, S-2o],
+        every class, for C > 2)."""
         self.submit(tiles_u8_host)
         return self.collect()
 

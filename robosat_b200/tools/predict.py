@@ -2,7 +2,8 @@
 robosat/tools/predict.py:23-113, with the batch loop replaced by the H100 path.
 
 Per batch the reference does H2D of fp32 tensors, DataParallel forward, softmax, D2H of B x 2 x S x S fp32, then
-crop / digitize / PNG on one CPU thread. Here: the dataset yields raw uint8 tiles, `TilePredictor` normalises,
+crop / digitize / PNG on one CPU thread. The reference handles 2-class models only (predict.py:98); for C > 2 classes every class
+plane c is written, in the same format, to `probs/<classes[c]>/z/x/y.png` (DESIGN.md §8). Here: the dataset yields raw uint8 tiles, `TilePredictor` normalises,
 runs the U-Net plan and the softmax / crop / quantise head on the GPU and returns uint8 bins; PNG encoding runs in
 a thread pool. With several GPUs the tile list is sharded by rank (one process per GPU), the checkpoint is
 broadcast once over NCCL and no other collective is used.
@@ -20,6 +21,7 @@ from PIL import Image
 from robosat_b200.colors import continuous_palette_for_color
 from robosat_b200.config import load_config
 from robosat_b200.datasets import BufferedSlippyMapDirectory
+from robosat_b200.tiles import _is_int
 from robosat_b200.transforms import ImageToUint8Tensor
 
 
@@ -42,6 +44,35 @@ def add_parser(subparser):
 
 NATIVE_PNG = os.environ.get("RSB_PNG_ENCODER", "native") != "pil"
 PNG_LEVEL = min(9, max(0, int(os.environ.get("RSB_PNG_LEVEL", "6"))))  # zlib level of the library encoder (3: ~40 % less encode time, files 4 - 16 % larger)
+
+
+def check_class_names(names):
+    """The dataset's class names become directory names under `probs` for a model of more than two classes: each must be a
+    non-empty, unique string without a path separator or NUL, not `.` or `..`, and not an integer (a directory `probs/<int>` would
+    be read as a zoom level by `tiles_from_slippy_map`). Raises ValueError naming the first bad class."""
+    seen = set()
+    for i, name in enumerate(names):
+        if not isinstance(name, str) or not name:
+            raise ValueError("class %d (%r) must be a non-empty string" % (i, name))
+        if any(ch in name for ch in ("/", "\\", "\0")):
+            raise ValueError("class %r must not contain a path separator or NUL" % name)
+        if name in (".", ".."):
+            raise ValueError("class %r is not a usable directory name" % name)
+        if _is_int(name):
+            raise ValueError("class %r is an integer and would be read as a zoom level" % name)
+        if name in seen:
+            raise ValueError("class %r appears more than once" % name)
+        seen.add(name)
+    return list(names)
+
+
+def _class_names(args, num_classes):
+    """None for a binary model (one probability directory, as the reference writes it); else the checked class names"""
+    if num_classes == 2:
+        return None
+    names = load_config(args.dataset)["common"]["classes"]
+    assert len(names) == num_classes, "dataset lists %d classes, the model has %d" % (len(names), num_classes)
+    return check_class_names(names)
 
 
 def _palette_bytes(palette):
@@ -72,21 +103,31 @@ def _save_png(root, palette, x, y, z, quantized, stats=None):
         stats["png_cpu_s"] = stats.get("png_cpu_s", 0.0) + (time.perf_counter() - t0)  # summed over pool threads (GIL-protected add)
 
 
-def _save_batch(root, palette, tiles, quantized, threads, stats=None):
+def _save_batch(root, palette, tiles, quantized, threads, stats=None, classes=None):
     """The PNG files of one batch through ONE library call (`rsb_png_write_p8_batch`: `threads` C++ threads, directories created
-    by the library); RSB_PNG_ENCODER=pil loops over `_save_png` with PIL instead. tiles: [(x, y, z)], quantized: uint8 [n, H, W]."""
+    by the library); RSB_PNG_ENCODER=pil loops over `_save_png` with PIL instead. tiles: [(x, y, z)], quantized: uint8 [n, H, W];
+    with `classes` (C > 2 names) quantized is uint8 [n, C, H, W] and plane c goes to root/classes[c]/z/x/y.png."""
     if not NATIVE_PNG:
         for (x, y, z), q in zip(tiles, quantized):
-            _save_png(root, palette, x, y, z, q, stats)
+            if classes is None:
+                _save_png(root, palette, x, y, z, q, stats)
+            else:
+                for name, plane in zip(classes, q):
+                    _save_png(os.path.join(root, name), palette, x, y, z, plane, stats)
         return
     import ctypes
 
     from robosat_b200 import _lib
 
     t0 = time.perf_counter()
-    n = len(tiles)
     pal = _palette_bytes(palette)
-    paths = (ctypes.c_char_p * n)(*[os.fsencode(os.path.join(root, str(z), str(x), str(y) + ".png")) for x, y, z in tiles])
+    if classes is None:
+        paths = [os.path.join(root, str(z), str(x), str(y) + ".png") for x, y, z in tiles]
+    else:  # (tile, class) order: the order of the planes in quantized
+        paths = [os.path.join(root, name, str(z), str(x), str(y) + ".png") for x, y, z in tiles for name in classes]
+        quantized = quantized.reshape(-1, *quantized.shape[2:])
+    n = len(paths)
+    paths = (ctypes.c_char_p * n)(*[os.fsencode(p) for p in paths])
     q = quantized if quantized.flags["C_CONTIGUOUS"] else quantized.copy()
     _lib.check(_lib.load().rsb_png_write_p8_batch(paths, n, q.ctypes.data, q.shape[1] * q.shape[2], q.shape[2], q.shape[1], pal, len(pal) // 3, PNG_LEVEL,
                                                   threads, 1), "rsb_png_write_p8_batch")
@@ -108,6 +149,7 @@ def run_shard(rank, world, args, device, sd, num_classes, stats=None):
     t_start = time.perf_counter()
     st = stats if stats is not None else {}
     tta = getattr(args, "tta", "none")  # Namespaces built by callers that predate the flag have no attribute
+    classes = _class_names(args, num_classes)
     size = args.tile_size + 2 * args.overlap
     palette = continuous_palette_for_color("pink", 256)
     # host cores of this rank -- min(affinity, cgroup CPU quota): the GPU boxes report 128 hardware threads under a quota of 16
@@ -164,7 +206,11 @@ def run_shard(rank, world, args, device, sd, num_classes, stats=None):
                 quantized = collect(predictor)
                 for tile, q in zip(tiles, quantized[:n]):
                     x, y, z = (int(v) for v in tile)
-                    pending.append(pool.submit(_save_png, args.probs, palette, x, y, z, q.copy(), st))
+                    if classes is None:
+                        pending.append(pool.submit(_save_png, args.probs, palette, x, y, z, q.copy(), st))
+                    else:
+                        for name, plane in zip(classes, q):
+                            pending.append(pool.submit(_save_png, os.path.join(args.probs, name), palette, x, y, z, plane.copy(), st))
             t0 = time.perf_counter()
             for f in pending:
                 f.result()
@@ -213,7 +259,7 @@ def run_shard(rank, world, args, device, sd, num_classes, stats=None):
                         coords = [(int(t.x), int(t.y), int(t.z)) for t in tiles]
                         bins = quantized[:len(tiles)].copy()
                         slots_free.release()
-                        pending.append(pool.submit(_save_batch, args.probs, palette, coords, bins, pool_threads, st))
+                        pending.append(pool.submit(_save_batch, args.probs, palette, coords, bins, pool_threads, st, classes))
                 except BaseException as exc:  # surfaced by the launching thread
                     failure.append(exc)
                     slots_free.release()
@@ -311,6 +357,12 @@ def _run(rank, world, args, port):
 
 
 def main(args):
+    names = load_config(args.dataset)["common"]["classes"]
+    if len(names) > 2:
+        try:
+            check_class_names(names)  # before any work: the names become directories under `probs`
+        except ValueError as exc:
+            sys.exit("Error: dataset %s: %s" % (args.dataset, exc))
     model = load_config(args.model)
     if not model["common"]["cuda"]:
         sys.exit("Error: robosat_b200 runs on CUDA devices only; set cuda = true in the model configuration")

@@ -7,7 +7,8 @@ batch of B tiles:
 
     expand:     one `rsb_augment_dihedral` launch per view writes the view's copy of the B tiles into its slice of the engine input
     per pass:   engine.forward (E = B*V/P tiles) -> `rsb_head_tta_accumulate` (softmax, inverse map, crop, int64 fixed-point sum)
-    finish:     `rsb_head_tta_quantize` (2 classes: np.digitize bins of the mean foreground) or `rsb_head_tta_argmax`
+    finish:     `rsb_head_tta_quantize` (2 classes: np.digitize bins of the mean foreground), `rsb_head_tta_quantize_classes` (every
+                class of a C > 2 model) or `rsb_head_tta_argmax`
 
 The chain is plain stream work, so a caller can capture it in a CUDA graph. The fixed-point sum makes the mean bit-identical
 however the views are ordered or split into passes.
@@ -98,11 +99,16 @@ class TtaChain:
         return self.acc
 
     def quantize(self, x, out_u8):
-        """2 classes: uint8 [B, H-2o, W-2o] np.digitize bins of the mean foreground probability"""
-        assert self.classes == 2, "single channel requires binary model"
+        """2 classes: uint8 [B, H-2o, W-2o] np.digitize bins of the mean foreground probability; C > 2: uint8 [B, C, H-2o, W-2o],
+        the bins of every class's mean probability"""
+        assert self.classes >= 2, "single channel requires binary model"
         self.accumulate(x)
-        _lib.check(_lib.load().rsb_head_tta_quantize(self.acc.data_ptr(), out_u8.data_ptr(), self.batch, self.OH * self.OW, self.V,
-                                                     _lib.current_stream_ptr()), "rsb_head_tta_quantize")
+        if self.classes == 2:
+            _lib.check(_lib.load().rsb_head_tta_quantize(self.acc.data_ptr(), out_u8.data_ptr(), self.batch, self.OH * self.OW, self.V,
+                                                         _lib.current_stream_ptr()), "rsb_head_tta_quantize")
+        else:
+            _lib.check(_lib.load().rsb_head_tta_quantize_classes(self.acc.data_ptr(), out_u8.data_ptr(), self.batch, self.classes, self.OH * self.OW,
+                                                                 self.V, _lib.current_stream_ptr()), "rsb_head_tta_quantize_classes")
         return out_u8
 
     def argmax(self, x, out_u8):
