@@ -507,6 +507,15 @@ int rsb_extract_valid(const int32_t* verts, const int64_t* ring_offsets, int32_t
  * depend on the launch shape. 1 <= M <= RSB_COMPARE_MAX_PLANES - 1; allocates nothing and does not synchronise. */
 #define RSB_COMPARE_MAX_PLANES 32
 int rsb_compare_count(const uint8_t* masks, const uint8_t* labels, int32_t N, int32_t M, int64_t hw, int64_t pitch, int64_t* counts, void* stream);
+/* rsb_compare_class_counts: the per-class agreement of `rs compare --csv --dataset`, on the planes of rsb_compare_count (same
+ * layout, pitch and alignment rules; labels NULL counts every label pixel as class 0). For C classes, 2 <= C <=
+ * RSB_COMPARE_MAX_CLASSES, it writes int64 label_hist [N][C] (pixels of label n equal to c), mask_hist [N][M][C] (pixels of mask
+ * (n, m) equal to c), both_hist [N][M][C] (pixels where label n == mask (n, m) == c) and out_of_range [N][1 + M] (pixels >= C in
+ * label n, then in each mask). Then tp = both, fp = mask - both, fn = label - both, tn = hw - label - mask + both per class.
+ * Integer sums, so the counts do not depend on the launch shape; allocates nothing and does not synchronise. */
+#define RSB_COMPARE_MAX_CLASSES 256
+int rsb_compare_class_counts(const uint8_t* masks, const uint8_t* labels, int32_t N, int32_t M, int32_t C, int64_t hw, int64_t pitch,
+                             int64_t* label_hist, int64_t* mask_hist, int64_t* both_hist, int64_t* out_of_range, void* stream);
 /* rsb_compare_compose: the side-by-side composite image | plane 0 | plane 1 | ... of N tiles of H x W. images uint8 [N][H][W][3]
  * (image n at images + n * H * W * 3); planes uint8 [N][P] index planes of H * W bytes at planes + (n * P + p) * pitch (plane 0 is
  * the label, planes 1.. the masks); palettes uint32 [N][P][256] (r | g << 8 | b << 16). out uint8 [N][H][(1 + P) * W][3], tile n

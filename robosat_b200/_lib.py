@@ -100,6 +100,7 @@ RSB_PBF_SEG_FIELDS = 16
  RSB_PBF_SEG_OUT_FIRST) = range(14)
 RSB_EXTRACT_WARP_RING = 256
 RSB_COMPARE_MAX_PLANES = 32
+RSB_COMPARE_MAX_CLASSES = 256
 
 
 class MorphOp(ctypes.Structure):
@@ -236,6 +237,7 @@ SIGNATURES = {
     "rsb_png_encode_rgb8": (_i64, [_vp, _i32, _i32, _i32, _vp, _i64]),
     "rsb_png_write_rgb8_batch": (ctypes.c_int, [_vp, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _i32]),
     "rsb_compare_count": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp]),
+    "rsb_compare_class_counts": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "rsb_compare_compose": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i64, _vp, _i64, _vp]),
     "rsb_softmax_nchw": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_cross_entropy": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),

@@ -8,7 +8,8 @@ mismatches are errors before anything is written), then tiles go in batches of o
 1. the masks (and, with a CSV, the labels) are decoded to index planes plus palettes by the library's PNG reader
    (`rsb_png_read_indexed_batch`, no interpreter lock), PIL's `convert("P")` for anything else;
 2. `rsb_compare_count` counts every mask's non-zero pixels and its confusion counts against the label; the coverage is that
-   integer count over W * H in float64 on the host, so the filter decides exactly as numpy does in the reference;
+   integer count over W * H in float64 on the host, so the filter decides exactly as numpy does in the reference; with the
+   dataset's classes, `rsb_compare_class_counts` adds the per-class histograms of the CSV on the same device planes;
 3. only kept tiles have their images (and labels) decoded; `rsb_compare_compose` expands the planes through their palettes and
    writes the composites into pinned host memory, which the library's RGB encoder writes out while the next batch decodes.
 """
@@ -33,6 +34,7 @@ NATIVE_DECODE = os.environ.get("RSB_PNG_DECODER", "native") != "pil"
 NATIVE_ENCODE = os.environ.get("RSB_PNG_ENCODER", "native") != "pil"
 PNG_LEVEL = min(9, max(0, int(os.environ.get("RSB_PNG_LEVEL", "6"))))
 CSV_COLUMNS = ["z", "x", "y", "mask", "coverage", "tp", "fp", "fn", "tn", "fg_iou"]
+CLASS_CSV_COLUMNS = ["z", "x", "y", "mask", "class", "coverage", "tp", "fp", "fn", "tn", "iou"]
 PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
 
 Job = namedtuple("Job", ["tile", "image", "label", "masks", "size"])
@@ -91,12 +93,13 @@ def _pil_indexed(path, plane, palette, size):
     palette.reshape(-1)[:len(pal)] = pal
 
 
-def decode_indexed(paths, planes, palettes, size, threads, pool=None):
+def decode_indexed(paths, planes, palettes, size, threads, pool=None, native_only=False):
     """`Image.open(p).convert("P")` of each path: index plane i into planes[i] (uint8, at least W * H bytes) and its colour table
     into palettes[i] (uint8 [256, 3]; entries past the file's palette are black, as PIL's convert("RGB") maps them). 8-bit gray
-    and palette PNGs go through ONE library call; anything it reports as unsupported, and every non-PNG file, through PIL."""
+    and palette PNGs go through ONE library call; anything it reports as unsupported, and every non-PNG file, through PIL.
+    `native_only`: every file goes through the library, and one it cannot decode is an RsbError naming it (no PIL)."""
     w, h = size
-    native = _native(paths)
+    native = list(range(len(paths))) if native_only else _native(paths)
     rest = sorted(set(range(len(paths))) - set(native))
     if native:
         n = len(native)
@@ -106,8 +109,9 @@ def decode_indexed(paths, planes, palettes, size, threads, pool=None):
         entries = np.empty(n, np.int32)
         rcs = (ctypes.c_int32 * n)()
         rc = _lib.load().rsb_png_read_indexed_batch(cpaths, n, outs, pals.ctypes.data, entries.ctypes.data, w, h, threads, rcs)
-        if rc != 0:
-            bad = [paths[native[k]] for k in range(n) if rcs[k] not in (0, _lib.RSB_E_UNSUPPORTED)]
+        if rc != 0 or (native_only and any(rcs)):
+            ok = (0,) if native_only else (0, _lib.RSB_E_UNSUPPORTED)
+            bad = [paths[native[k]] for k in range(n) if rcs[k] not in ok]
             raise _lib.RsbError("decoding %s failed (rc=%d): %s" % (bad[:3], rc, _lib.last_error()))
         for k, i in enumerate(native):
             if rcs[k] == 0:
@@ -169,6 +173,21 @@ def count_device(masks, labels, hw, counts=None):
     return counts
 
 
+def class_counts_device(masks, labels, hw, num_classes, out=None):
+    """masks: uint8 CUDA tensor [N, M, pitch]; labels: uint8 CUDA tensor [N, pitch] or None (all class 0) -> int64 CUDA tensors
+    (label_hist [N, C], mask_hist [N, M, C], both_hist [N, M, C], out_of_range [N, 1 + M]) of `rsb_compare_class_counts`, written
+    into `out` (a tuple of the same four) when given. Enqueued on the current stream."""
+    import torch
+
+    N, M, pitch = masks.shape
+    C = num_classes
+    if out is None:
+        out = tuple(_alloc(shape, torch.int64, masks.device, "the class counts of %d tiles" % N) for shape in ((N, C), (N, M, C), (N, M, C), (N, 1 + M)))
+    _lib.check(_lib.load().rsb_compare_class_counts(masks.data_ptr(), labels.data_ptr() if labels is not None else None, N, M, C, hw, pitch,
+                                                    *(t.data_ptr() for t in out), _lib.current_stream_ptr()), "rsb_compare_class_counts")
+    return out
+
+
 def compose_device(images, planes, palettes, size, out):
     """images: uint8 CUDA tensor [N, H * W * 3]; planes: uint8 CUDA tensor [N, P, pitch] (label, then masks); palettes: uint32
     CUDA tensor [N, P, 256]; out: uint8 tensor [N, stride] in pinned host or device memory -> out[n, :H * (1 + P) * W * 3] is
@@ -179,20 +198,20 @@ def compose_device(images, planes, palettes, size, out):
                                                out.stride(0), _lib.current_stream_ptr()), "rsb_compare_compose")
 
 
-def tile_bytes(size, M, with_labels):
-    """device plus pinned host bytes one tile of a batch needs"""
+def tile_bytes(size, M, with_labels, num_classes=0):
+    """device plus pinned host bytes one tile of a batch needs; `num_classes` > 0 adds the per-class counts (3 * C int64 per mask)"""
     hw = size[0] * size[1]
     pitch = pitch_of(hw)
     device = M * pitch + (pitch if with_labels else 0) + M * 32 + 3 * hw + (1 + M) * (pitch + 1024) + pitch
-    return device + out_stride_of(size, 1 + M)
+    return device + out_stride_of(size, 1 + M) + M * 3 * num_classes * 8
 
 
-def batches(jobs, M, with_labels, budget):
+def batches(jobs, M, with_labels, budget, num_classes=0):
     """runs of consecutive jobs of one size whose tile_bytes fit in `budget` (one tile at least, 65535 at most)"""
     start = 0
     while start < len(jobs):
         size = jobs[start].size
-        cap = min(65535, max(1, budget // tile_bytes(size, M, with_labels)))
+        cap = min(65535, max(1, budget // tile_bytes(size, M, with_labels, num_classes)))
         end = start + 1
         while end < len(jobs) and end - start < cap and jobs[end].size == size:
             end += 1
@@ -211,12 +230,39 @@ def csv_rows(batch, counts, coverage):
     return rows
 
 
-def write_csv(path, rows):
+def class_csv_rows(batch, label_hist, mask_hist, both_hist, coverage, classes, hw):
+    """`CLASS_CSV_COLUMNS` rows of a batch, one per (tile, mask, class) with the classes in dataset order: label_hist int64 [N, C],
+    mask_hist and both_hist int64 [N, M, C], coverage float64 [N, M]; tp = both, fp = mask - both, fn = label - both,
+    tn = hw - label - mask + both, iou = tp / (tp + fp + fn), empty when that is 0"""
+    rows = []
+    for j, lab, msk, both, cov in zip(batch, label_hist, mask_hist, both_hist, coverage):
+        for m in range(len(msk)):
+            for c, name in enumerate(classes):
+                tp, mk, lb = int(both[m, c]), int(msk[m, c]), int(lab[c])
+                fp, fn = mk - tp, lb - tp
+                union = tp + fp + fn
+                rows.append([j.tile.z, j.tile.x, j.tile.y, m, name, repr(float(cov[m])), tp, fp, fn, hw - lb - mk + tp,
+                             repr(tp / union) if union else ""])
+    return rows
+
+
+def out_of_range_error(batch, out_of_range, num_classes):
+    """CompareError for the first tile of the batch whose label or a mask holds a value >= C (out_of_range int64 [N, 1 + M]), or None"""
+    for j, row in zip(batch, out_of_range):
+        for p, count in enumerate(row):
+            if count:
+                path = j.label if p == 0 else j.masks[p - 1]
+                return CompareError("tile %s/%s/%s: %s holds %d pixels with a value outside the dataset's %d classes 0..%d"
+                                    % (j.tile.z, j.tile.x, j.tile.y, path, int(count), num_classes, num_classes - 1))
+    return None
+
+
+def write_csv(path, rows, columns=CSV_COLUMNS):
     import csv
 
     with open(path, "w", newline="") as fp:
         writer = csv.writer(fp)
-        writer.writerow(CSV_COLUMNS)
+        writer.writerow(columns)
         writer.writerows(rows)
 
 
@@ -241,18 +287,27 @@ def write_composites(paths, out, size, columns, threads):
                "rsb_png_write_rgb8_batch")
 
 
-def compare_device(images, labels, masks, out, minimum=0.0, maximum=1.0, csv=None, budget=DEFAULT_BUDGET, stats=None, device=None):
-    """`rs compare images labels masks... --minimum --maximum [--csv]`: writes out/z/x/y.png for every tile with at least one
-    mask whose coverage p satisfies minimum <= p <= maximum, and the CSV of every (tile, mask) when `csv` is a path.
+def compare_device(images, labels, masks, out, minimum=0.0, maximum=1.0, csv=None, budget=DEFAULT_BUDGET, stats=None, device=None,
+                   classes=None):
+    """`rs compare images labels masks... --minimum --maximum [--csv [--dataset]]`: writes out/z/x/y.png for every tile with at
+    least one mask whose coverage p satisfies minimum <= p <= maximum, and the CSV of every (tile, mask) when `csv` is a path.
+    With `classes` (the dataset's class names, which needs `csv`) the CSV has `CLASS_CSV_COLUMNS`, one row per (tile, mask, class),
+    counted by `rsb_compare_class_counts` in the same pass as the coverage; a label or mask value >= C is a CompareError naming the
+    tile and the file. The coverage filter and the composites do not change.
 
     `stats` (a dict) receives decode_s / device_s / encode_s (wall seconds on the calling thread; encode_s on the encode thread),
-    wait_s (the calling thread waiting for the previous batch's encode), kernel_ms (CUDA events around the two kernels), tiles, kept and written. CompareError before anything is written when a tile
+    wait_s (the calling thread waiting for the previous batch's encode), kernel_ms (CUDA events around the kernels), tiles, kept and written. CompareError before anything is written when a tile
     cannot be compared."""
     import torch
 
     M = len(masks)
     if not 1 <= M < _lib.RSB_COMPARE_MAX_PLANES - 1:
         raise CompareError("between 1 and %d mask directories are supported, got %d" % (_lib.RSB_COMPARE_MAX_PLANES - 2, M))
+    if classes is not None and not csv:
+        raise CompareError("per-class counts are written to the CSV: classes need a csv path")
+    C = len(classes) if classes is not None else 0
+    if classes is not None and not 2 <= C <= _lib.RSB_COMPARE_MAX_CLASSES:
+        raise CompareError("between 2 and %d classes are supported, got %d" % (_lib.RSB_COMPARE_MAX_CLASSES, C))
     jobs = plan(images, labels, masks)
     dev = torch.device(device if device is not None else "cuda")
     st = stats if stats is not None else {}
@@ -272,7 +327,7 @@ def compare_device(images, labels, masks, out, minimum=0.0, maximum=1.0, csv=Non
 
     with ThreadPoolExecutor(max_workers=threads) as pool, ThreadPoolExecutor(max_workers=1) as encoder:
         pending = None
-        for batch in batches(jobs, M, csv is not None, budget):
+        for batch in batches(jobs, M, csv is not None, budget, C):
             B, size = len(batch), batch[0].size
             hw = size[0] * size[1]
             pitch = pitch_of(hw)
@@ -298,12 +353,19 @@ def compare_device(images, labels, masks, out, minimum=0.0, maximum=1.0, csv=Non
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             count_device(d_masks, d_labels, hw, counts)
+            hists = class_counts_device(d_masks, d_labels, hw, C) if C else None
             e1.record()
             events.append((e0, e1))
             counts = counts.cpu().numpy()
             coverage = (counts[..., 0] + counts[..., 1]) / np.int64(hw)  # float64, as np.sum(...) / np.prod(image.size)
             keep = ((coverage >= minimum) & (coverage <= maximum)).any(axis=1)
-            if rows is not None:
+            if hists is not None:
+                label_hist, mask_hist, both_hist, out_of_range = (t.cpu().numpy() for t in hists)
+                err = out_of_range_error(batch, out_of_range, C)
+                if err is not None:
+                    raise err
+                rows.extend(class_csv_rows(batch, label_hist, mask_hist, both_hist, coverage, classes, hw))
+            elif rows is not None:
                 rows.extend(csv_rows(batch, counts, coverage))
             t2 = time.perf_counter()
             st["device_s"] += t2 - t1
@@ -352,5 +414,5 @@ def compare_device(images, labels, masks, out, minimum=0.0, maximum=1.0, csv=Non
     torch.cuda.synchronize(dev)
     st["kernel_ms"] = sum(a.elapsed_time(b) for a, b in events)
     if csv:
-        write_csv(csv, rows)
+        write_csv(csv, rows, CLASS_CSV_COLUMNS if C else CSV_COLUMNS)
     return st
