@@ -290,6 +290,22 @@ typedef struct rsb_morph_op {
 int rsb_morph_binary(const uint8_t* labels, int64_t image_stride, int32_t N, int32_t H, int32_t W, int32_t class_index,
                      const rsb_morph_op* ops_host, int32_t nops, uint8_t* out, int32_t* fg_counts, void* stream);
 
+/* `rs features --type building` connected components (the rule is DESIGN.md §8). planes uint8 [N] images of H x W, image n at
+ * planes + n * image_stride; the outputs are int32 [N][H][W]. 1 <= N <= 65535, 1 <= H, W <= RSB_LABEL_MAX_SIZE. Labels are
+ * image-local pixel indices y * W + x: labels[n][y][x] = the smallest index of the pixel's component of (plane == value) under
+ * 4- or 8-connectivity (`connectivity` = 4 or 8), -1 off the plane; areas[n][y][x] = the number of pixels of that component, 0 off
+ * the plane. Identical on every run. Arguments are validated before the device check; allocates nothing and does not synchronise. */
+#define RSB_LABEL_MAX_SIZE 8192
+int rsb_label_components(const uint8_t* planes, int64_t image_stride, int32_t N, int32_t H, int32_t W, int32_t value, int32_t connectivity,
+                         int32_t* labels, int32_t* areas, void* stream);
+/* Speck drop and hole fill of the building rule on `opened` ({0, 1} images laid out as rsb_label_components' planes, e.g. the
+ * opening from rsb_morph_binary): D = the pixels of 8-connected foreground components of at least min_area pixels; out uint8
+ * {0, 1} [N][H][W] = D plus every 4-connected background component of D that touches no image border and has fewer than
+ * min_hole_area pixels; fg_counts int32 [N] = the 1 pixels of each result. labels, stats: int32 [N][H][W] workspaces (not
+ * aliased). Same limits and guarantees as rsb_label_components. */
+int rsb_building_clean(const uint8_t* opened, int64_t image_stride, int32_t N, int32_t H, int32_t W, int32_t min_area, int32_t min_hole_area,
+                       int32_t* labels, int32_t* stats, uint8_t* out, int32_t* fg_counts, void* stream);
+
 /* `rs rasterize` polygon fill (robosat/tools/rasterize.py:64-83: rasterio.features.rasterize, all_touched=False, burn value 1,
  * merge "replace"). All arrays are DEVICE pointers. Polygons: vertices float64 [num_vertices][2] (EPSG:3857 X, Y; 16-byte aligned);
  * ring r owns vertices [ring_offsets[r], ring_offsets[r + 1]) and is closed implicitly; polygon p owns rings

@@ -6,6 +6,10 @@ bit-identical to OpenCV. The launch also counts each result's foreground, so emp
 simplification and the hierarchy walk stay on the host with the reference's OpenCV calls. The ring order, the three warnings and
 the skips are the reference's. `mercantile` and `shapely` are not needed: `bounds` restates mercantile's tile bounds, and
 `polygon_is_valid` restates the OGC validity rules that the reference asks shapely for.
+
+`BuildingHandler` is this project's building rule (the reference has none; DESIGN.md §8): a small opening, then connected
+components on the device (`rsb_building_clean`) drop specks and fill small holes, and the host turns each outer contour and its
+holes into one polygon.
 """
 
 import collections
@@ -77,6 +81,59 @@ def morph_device(labels, class_index, ops):
     counts = torch.empty((N,), dtype=torch.int32, device=labels.device)
     _lib.check(_lib.load().rsb_morph_binary(labels.data_ptr(), labels.stride(0) if N > 1 else H * W, N, H, W, int(class_index), arr, len(ops),
                                             out.data_ptr(), counts.data_ptr(), _lib.current_stream_ptr()), "rsb_morph_binary")
+    return out, counts
+
+
+def _planes(planes, what):
+    import torch
+
+    if not planes.is_cuda or planes.dtype != torch.uint8 or planes.dim() != 3:
+        raise ValueError("%s needs a uint8 CUDA tensor [N, H, W]" % what)
+    N, H, W = planes.shape
+    if planes.stride(2) != 1 or planes.stride(1) != W:
+        raise ValueError("%s needs contiguous rows of each image" % what)
+    return N, H, W, planes.stride(0) if N > 1 else H * W
+
+
+def components_device(planes, value, connectivity):
+    """planes: uint8 CUDA tensor [N, H, W] (rows contiguous) -> (int32 [N, H, W] root of each pixel's component of
+    (planes == value) under 4- or 8-connectivity, i.e. its smallest pixel index y * W + x in the image, or -1 off the plane;
+    int32 [N, H, W] the area of that component, 0 off the plane). Enqueued on the current stream, no synchronisation."""
+    import torch
+
+    from robosat_b200.cover import _alloc
+
+    N, H, W, stride = _planes(planes, "components_device")
+    labels = _alloc((N, H, W), torch.int32, planes.device, "component labels")
+    areas = _alloc((N, H, W), torch.int32, planes.device, "component areas")
+    _lib.check(_lib.load().rsb_label_components(planes.data_ptr(), stride, N, H, W, int(value), int(connectivity), labels.data_ptr(),
+                                                areas.data_ptr(), _lib.current_stream_ptr()), "rsb_label_components")
+    return labels, areas
+
+
+def building_open(k_denoise=5):
+    """The building rule's denoise: MORPH_OPEN with a k x k ellipse = erode, dilate."""
+    return [ellipse_op(k_denoise, False), ellipse_op(k_denoise, True)]
+
+
+def building_clean_device(labels, class_index, k_denoise=5, min_area=64, min_hole_area=64):
+    """labels: uint8 CUDA tensor [N, H, W] of class indices -> (uint8 [N, H, W] {0, 1} cleaned building masks, int32 [N] foreground
+    counts), both on the device: the opening of (labels == class_index), then 8-connected components below min_area pixels dropped,
+    then 4-connected background components below min_hole_area pixels that miss the tile border filled (DESIGN.md §8). Enqueued
+    on the current stream, no synchronisation."""
+    import torch
+
+    from robosat_b200.cover import _alloc
+
+    opened, _ = morph_device(labels, class_index, building_open(k_denoise))
+    N, H, W = opened.shape
+    work = _alloc((N, H, W), torch.int32, opened.device, "building component labels")
+    stats = _alloc((N, H, W), torch.int32, opened.device, "building component areas")
+    out = torch.empty((N, H, W), dtype=torch.uint8, device=opened.device)
+    counts = torch.empty((N,), dtype=torch.int32, device=opened.device)
+    _lib.check(_lib.load().rsb_building_clean(opened.data_ptr(), H * W, N, H, W, int(min_area), int(min_hole_area), work.data_ptr(),
+                                              stats.data_ptr(), out.data_ptr(), counts.data_ptr(), _lib.current_stream_ptr()),
+               "rsb_building_clean")
     return out, counts
 
 
@@ -356,3 +413,68 @@ class ParkingHandler:
     def save(self, out):
         with open(out, "w") as fp:
             json.dump({"type": "FeatureCollection", "features": self.features}, fp)
+
+
+# --- buildings (this project's rule; the reference has no building handler: DESIGN.md §8) ----------------------------------------
+
+def polygons_from_filled(tile, filled, simplify_epsilon=1.0):
+    """Host half of `BuildingHandler`: one Polygon per outer contour of a cleaned {0, 1} uint8 mask, with its holes.
+
+    Contours are `cv2.findContours(RETR_CCOMP, CHAIN_APPROX_SIMPLE)`: outer contours in OpenCV's order, each followed by its child
+    holes in list order. Every ring is simplified with `approxPolyDP(epsilon=simplify_epsilon)`; when a simplified ring has fewer
+    than 3 vertices or the simplified polygon is not valid, the traced rings are used, and when those are not valid either the
+    polygon is skipped with W_INVALID. Returns (features, warnings); thread-safe, as `polygons_from_grown`."""
+    import cv2
+
+    features, warnings = [], []
+    contours, hierarchy = cv2.findContours(filled, cv2.RETR_CCOMP, cv2.CHAIN_APPROX_SIMPLE)
+    if hierarchy is None:
+        return features, warnings
+    parents = hierarchy[0][:, 3]
+    for outer in np.flatnonzero(parents == -1):
+        ring_ids = [outer] + [int(h) for h in np.flatnonzero(parents == outer)]
+        traced = [[tuple(int(v) for v in pt[0]) for pt in contours[r]] for r in ring_ids]
+        simplified = [[tuple(int(v) for v in pt[0]) for pt in cv2.approxPolyDP(contours[r], simplify_epsilon, True)] for r in ring_ids]
+        if all(len(r) >= 3 for r in simplified) and polygon_is_valid(simplified):
+            rings = simplified
+        elif polygon_is_valid(traced):
+            rings = traced
+        else:
+            warnings.append(W_INVALID)
+            continue
+        coords = [featurize(tile, ring, filled.shape[:2]) for ring in rings]
+        features.append({"type": "Feature", "geometry": {"type": "Polygon", "coordinates": coords}, "properties": {}})
+    return features, warnings
+
+
+class BuildingHandler(ParkingHandler):
+    """Building footprints: `apply(tile, mask)` per tile, `apply_batch` for a batch of label images on the device, `save(out)`.
+
+    The mask cleanup (an opening with a k_denoise x k_denoise ellipse, speck drop, small-hole fill) runs on the device in
+    `building_clean_device`; the contours run on the host in `polygons_from_filled`. The thresholds are this project's choices
+    for z18 tiles of 512 px (64 px is about 2.4 m square there), not tuned against imagery."""
+
+    kernel_size_denoise = 5
+    min_area = 64
+    min_hole_area = 64
+    simplify_epsilon = 1.0
+
+    def check_zoom(self, tile):
+        if tile.z != 18:
+            raise NotImplementedError("Building post-processing thresholds are set for z18")
+
+    def apply_batch(self, tiles, labels_device, class_index, pool=None):
+        """tiles: N tiles; labels_device: uint8 CUDA tensor [N, H, W] of class indices. Features of (labels == class_index) are
+        appended in tile order. Tiles whose cleaned mask is empty do no host work. `pool` (an Executor) runs the contour step."""
+        for t in tiles:
+            self.check_zoom(t)
+        filled, counts = building_clean_device(labels_device, class_index, self.kernel_size_denoise, self.min_area, self.min_hole_area)
+        full = np.flatnonzero(counts.cpu().numpy())
+        if len(full) == 0:
+            return
+        import torch
+
+        masks = filled[torch.from_numpy(full).to(filled.device)].cpu().numpy()
+        work = [(tiles[i], m) for i, m in zip(full, masks)]
+        run = lambda tm: polygons_from_filled(tm[0], tm[1], self.simplify_epsilon)  # noqa: E731
+        self._gather(pool.map(run, work) if pool is not None else map(run, work))

@@ -1,8 +1,9 @@
 """`rs features` (robosat/tools/features.py): simplified GeoJSON features from segmentation masks.
 
-Same flags and output. Masks are decoded in a thread pool, batches of same-size tiles go to the device for the morphology
-(`robosat_b200.features.ParkingHandler.apply_batch`), and the contour step of non-empty tiles runs in the same pool. Tiles are
-processed in (z, x, y) order, so features come out in that order rather than in directory-listing order."""
+Same flags and output, plus `--type building` (this project's rule, `robosat_b200.features.BuildingHandler`). Masks are decoded
+in a thread pool, batches of same-size tiles go to the device for the mask cleanup (the handler's `apply_batch`), and the contour
+step of non-empty tiles runs in the same pool. Tiles are processed in (z, x, y) order, so features come out in that order rather
+than in directory-listing order. `--type` must be one of the dataset's classes."""
 
 import argparse
 import sys
@@ -12,11 +13,11 @@ import numpy as np
 from PIL import Image
 
 from robosat_b200.config import load_config
-from robosat_b200.features import ParkingHandler
+from robosat_b200.features import BuildingHandler, ParkingHandler
 from robosat_b200.hostinfo import usable_cores
 from robosat_b200.tiles import tiles_from_slippy_map
 
-handlers = {"parking": ParkingHandler}
+handlers = {"parking": ParkingHandler, "building": BuildingHandler}
 
 
 def add_parser(subparser):
@@ -49,7 +50,8 @@ def main(args, batch=64):
 
     dataset = load_config(args.dataset)
     labels = dataset["common"]["classes"]
-    assert set(labels).issuperset(set(handlers.keys())), "handlers have a class label"
+    if args.type not in labels:
+        sys.exit("Error: rs features --type %s needs a class %r in the dataset's classes %s" % (args.type, args.type, labels))
     index = labels.index(args.type)
     try:
         import cv2  # noqa: F401
