@@ -587,6 +587,41 @@ int rsb_png_write_rgb8_batch(const char* const* paths, int32_t n, const uint8_t*
                              int32_t level, int32_t threads, int32_t make_dirs);
 
 /* ---------------------------------------------------------------------------------------------
+ * `rs tile`: slippy-map RGB tiles from a GeoTIFF (the rule is DESIGN.md §8; robosat_b200/tile.py plans the work).
+ */
+/* Decode raster rows [row0, row0 + rows) x columns [col0, col0 + cols) of an 8-bit chunky (PlanarConfiguration 1) TIFF image into
+ * out_host uint8 [rows][cols][spp], on `threads` threads of the library's own. file_host: the file's bytes [file_len] (e.g. a memory
+ * map); chunk i (strip, or tile in row-major order) is file_host[chunk_offsets_host[i] .. + chunk_bytes_host[i]). tiled = 0: strips
+ * of chunk_h rows (chunk_w = width; the last strip holds the remaining rows); tiled = 1: tiles of chunk_w x chunk_h, ragged tiles
+ * stored whole. spp 1, 3 or 4; compression 1 (none), 5 (LZW), 8 or 32946 (zlib DEFLATE); predictor 1 or 2 (horizontal
+ * differencing). Only the chunks the window touches are read. A chunk that cannot be decoded (outside the file, too short, truncated
+ * or corrupt stream, bad LZW code) gives RSB_E_INVALID with a message naming the strip or tile and *bad_chunk_host = its index
+ * (-1 otherwise; bad_chunk_host may be NULL). Host only: no device needed. */
+int rsb_tiff_decode_window(const uint8_t* file_host, int64_t file_len, const int64_t* chunk_offsets_host, const int64_t* chunk_bytes_host,
+                           int64_t num_chunks, int64_t width, int64_t height, int32_t chunk_w, int32_t chunk_h, int32_t tiled, int32_t spp,
+                           int32_t compression, int32_t predictor, int64_t row0, int64_t rows, int64_t col0, int64_t cols, uint8_t* out_host,
+                           int32_t threads, int64_t* bad_chunk_host);
+
+/* Warp N tiles of size x size of zoom z from a source window. src uint8 [win_rows][src_pitch] holds raster rows
+ * [win_row0, + win_rows) x columns [win_col0, + win_cols) of a raster_w x raster_h image, spp (1, 3 or 4) samples per pixel (spp = 4:
+ * 4-byte aligned rows). A pixel is valid unless alpha = 1 and its 4th sample is 0, or its colour samples (1 or 3) all equal nodata
+ * (-1: none). nodes float64 [nodes_h][nodes_w][2] (16-byte aligned): the source coordinates (u, v) of global tile pixel centres
+ * (kG + 1/2, lG + 1/2) for k = node_x0 + column, l = node_y0 + row, G = grid_step (a power of two <= RSB_TILE_MAX_STEP). tiles
+ * int64 [N][2] = (x, y); pixel (c, r) of tile n is global pixel (x S + c, y S + r) and interpolates the four nodes of its lattice
+ * cell with weights (g - kG) / G, then samples: nearest (resampling 0) or bilinear (1), per DESIGN.md §8; every float64 operation
+ * rounded separately. out uint8 RGB [N][size][size][3] at out + n * image_stride; an uncovered pixel is (0, 0, 0). covered int64
+ * [N] = covered pixels per tile; misses int64 [1] = samples inside the raster but outside the window, plus pixels whose lattice
+ * cell lies outside `nodes` (0 unless the host planned wrongly; such pixels are left uncovered). Both are cleared by the call.
+ * 1 <= N <= 65535, 1 <= size <= RSB_TILE_MAX_SIZE. Arguments are validated before the device check; allocates nothing and does
+ * not synchronise. */
+#define RSB_TILE_MAX_SIZE 4096
+#define RSB_TILE_MAX_STEP 64
+int rsb_tile_warp(const uint8_t* src, int64_t src_pitch, int64_t win_row0, int64_t win_col0, int64_t win_rows, int64_t win_cols,
+                  int64_t raster_w, int64_t raster_h, int32_t spp, int32_t alpha, int32_t nodata, const double* nodes, int64_t node_x0,
+                  int64_t node_y0, int32_t nodes_w, int32_t nodes_h, int32_t grid_step, const int64_t* tiles, int32_t N, int32_t size,
+                  int32_t resampling, uint8_t* out, int64_t image_stride, int64_t* covered, int64_t* misses, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Losses and metrics on fp32 NCHW logits + int64 targets [N][H][W].
  */
 /* CrossEntropyLoss2d.forward (losses.py:24-25): weighted NLL of log_softmax, mean over sum of target weights.

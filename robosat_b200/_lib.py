@@ -102,6 +102,8 @@ RSB_PBF_SEG_FIELDS = 16
 RSB_EXTRACT_WARP_RING = 256
 RSB_COMPARE_MAX_PLANES = 32
 RSB_COMPARE_MAX_CLASSES = 256
+RSB_TILE_MAX_SIZE = 4096
+RSB_TILE_MAX_STEP = 64
 
 
 class MorphOp(ctypes.Structure):
@@ -239,6 +241,10 @@ SIGNATURES = {
     "rsb_png_read_indexed_batch": (ctypes.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "rsb_png_encode_rgb8": (_i64, [_vp, _i32, _i32, _i32, _vp, _i64]),
     "rsb_png_write_rgb8_batch": (ctypes.c_int, [_vp, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _i32]),
+    "rsb_tiff_decode_window": (ctypes.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64,
+                                              _vp, _i32, _vp]),
+    "rsb_tile_warp": (ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _vp, _i32,
+                                     _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
     "rsb_compare_count": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp]),
     "rsb_compare_class_counts": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "rsb_compare_compose": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i64, _vp, _i64, _vp]),
