@@ -621,6 +621,30 @@ int rsb_tile_warp(const uint8_t* src, int64_t src_pitch, int64_t win_row0, int64
                   int64_t node_y0, int32_t nodes_w, int32_t nodes_h, int32_t grid_step, const int64_t* tiles, int32_t N, int32_t size,
                   int32_t resampling, uint8_t* out, int64_t image_stride, int64_t* covered, int64_t* misses, void* stream);
 
+/* rs mosaic (DESIGN.md §8): deflate the chunk x chunk tiles of one row of a 1-band 8-bit raster window. window_host uint8 rows x cols
+ * (row pitch `pitch`, rows <= chunk); tile k holds columns [k chunk, (k + 1) chunk) and is padded with `fill` past the window's rows
+ * and columns, then zlib-compressed (compress2 at `level`) into out_host + k * chunk_cap; sizes_host int64 [ceil(cols / chunk)] gets
+ * the compressed byte counts. chunk_cap >= rsb_tiff_deflate_bound(chunk * chunk). Tiles are compressed on `threads` of the library's
+ * threads. Host only: no device needed. */
+int64_t rsb_tiff_deflate_bound(int64_t n);
+int rsb_tiff_encode_chunks(const uint8_t* window_host, int64_t pitch, int32_t rows, int32_t cols, int32_t chunk, int32_t fill, int32_t level,
+                           uint8_t* out_host, int64_t chunk_cap, int64_t* sizes_host, int32_t threads);
+
+/* rs mosaic (DESIGN.md §8): slippy-map index tiles of zoom `zoom` (size x size) sampled onto a window of an output raster. planes uint8
+ * [num_planes] x plane_stride: the decoded index planes (row-major size x size). slots int32 [tiles_h][tiles_w]: the plane of tile
+ * (tile_x0 + column, tile_y0 + row), -1 when it has no file. nodes float64 [nodes_h][nodes_w][2] (16-byte aligned): the global
+ * pixel coordinates (gx, gy) of the centres of output pixels (kG, lG), k = node_x0 + column, l = node_y0 + row, G = grid_step (a power
+ * of two <= RSB_TILE_MAX_STEP). Output pixel (out_col0 + c, out_row0 + r), 0 <= c < out_cols, 0 <= r < out_rows, interpolates the
+ * four nodes of its lattice cell with weights (i - kG) / G and samples nearest (resampling 0) or bilinear (1), per DESIGN.md §8, every
+ * float64 operation rounded separately; it is written to out + r * out_pitch + c, `nodata` (0..255) when uncovered. covered int64 [1]
+ * = covered pixels; misses int64 [1] = samples inside the world but outside the slot table, plus pixels whose lattice cell lies
+ * outside `nodes` (0 unless the host planned wrongly; such pixels are left uncovered). Both are cleared by the call. Arguments are
+ * validated before the device check; allocates nothing and does not synchronise. */
+int rsb_mosaic_warp(const uint8_t* planes, int64_t plane_stride, int32_t num_planes, const int32_t* slots, int64_t tile_x0, int64_t tile_y0,
+                    int32_t tiles_w, int32_t tiles_h, int32_t zoom, int32_t size, const double* nodes, int64_t node_x0, int64_t node_y0,
+                    int32_t nodes_w, int32_t nodes_h, int32_t grid_step, int64_t out_col0, int64_t out_row0, int32_t out_cols, int32_t out_rows,
+                    int32_t resampling, int32_t nodata, uint8_t* out, int64_t out_pitch, int64_t* covered, int64_t* misses, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Losses and metrics on fp32 NCHW logits + int64 targets [N][H][W].
  */

@@ -245,6 +245,10 @@ SIGNATURES = {
                                               _vp, _i32, _vp]),
     "rsb_tile_warp": (ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _vp, _i32,
                                      _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
+    "rsb_tiff_deflate_bound": (_i64, [_i64]),
+    "rsb_tiff_encode_chunks": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i32]),
+    "rsb_mosaic_warp": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _i64, _i64,
+                                       _i32, _i32, _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
     "rsb_compare_count": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i64, _i64, _vp, _vp]),
     "rsb_compare_class_counts": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "rsb_compare_compose": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i64, _vp, _i64, _vp]),

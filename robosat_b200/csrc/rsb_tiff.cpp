@@ -1,5 +1,6 @@
-// Host side of `rs tile` (DESIGN.md §8): decoding a window of an 8-bit chunky TIFF's strips or tiles into a caller's buffer.
-// Plain C++, no Python, no interpreter lock; the chunks a window touches are decoded on the library's own threads.
+// Host side of `rs tile` and `rs mosaic` (DESIGN.md §8): decoding a window of an 8-bit chunky TIFF's strips or tiles into a caller's
+// buffer, and deflating the square tiles of a window of a 1-band 8-bit raster. Plain C++, no Python, no interpreter lock; the chunks
+// of a window are decoded or compressed on the library's own threads.
 //
 // The IFD and GeoKey parsing stay in Python (robosat_b200/geotiff.py); this file sees the raster through its chunk table. Each chunk
 // is decoded into a per-thread scratch (inflate through the library's DEFLATE decoder, or LZW), predictor 2 is undone on its rows,
@@ -15,6 +16,7 @@
 #include "../../include/rsb200.h"
 #include "rsb_host.h"
 #include "rsb_inflate.h"
+#include <zlib.h>
 
 using rsb::set_error;
 
@@ -209,5 +211,34 @@ extern "C" int rsb_tiff_decode_window(const uint8_t* file, int64_t file_len, con
         return set_error(RSB_E_INVALID, "tiff_decode_window: %s %lld (offset %lld, %lld bytes): %s", tiled ? "tile" : "strip", (long long)idx,
                          (long long)chunk_offsets[idx], (long long)chunk_bytes[idx], chunk_error_text(rc[size_t(k)]));
     }
+    return RSB_OK;
+}
+
+extern "C" int64_t rsb_tiff_deflate_bound(int64_t n) { return n < 0 ? -1 : int64_t(compressBound(uLong(n))); }
+
+extern "C" int rsb_tiff_encode_chunks(const uint8_t* window, int64_t pitch, int32_t rows, int32_t cols, int32_t chunk, int32_t fill, int32_t level,
+                                      uint8_t* out, int64_t chunk_cap, int64_t* sizes, int32_t threads) {
+    if (!window || !out || !sizes) return set_error(RSB_E_INVALID, "tiff_encode_chunks: null pointer");
+    if (chunk < 16 || chunk > 4096 || chunk % 16) return set_error(RSB_E_INVALID, "tiff_encode_chunks: chunk %d (need a multiple of 16 in 16..4096)", chunk);
+    if (rows < 1 || rows > chunk || cols < 1 || pitch < cols)
+        return set_error(RSB_E_INVALID, "tiff_encode_chunks: window %d x %d, pitch %lld, chunk %d", cols, rows, (long long)pitch, chunk);
+    if (fill < 0 || fill > 255 || level < 0 || level > 9) return set_error(RSB_E_INVALID, "tiff_encode_chunks: fill %d, level %d", fill, level);
+    const size_t raw = size_t(chunk) * size_t(chunk);
+    if (chunk_cap < int64_t(compressBound(uLong(raw))))
+        return set_error(RSB_E_INVALID, "tiff_encode_chunks: %lld bytes per chunk, compressBound needs %lld", (long long)chunk_cap,
+                         (long long)compressBound(uLong(raw)));
+    const int64_t n = (int64_t(cols) + chunk - 1) / chunk;
+    std::vector<int> rc(size_t(n), Z_OK);
+    parallel_for(n, threads, [&](int64_t k) {
+        static thread_local std::vector<uint8_t> buf;
+        buf.assign(raw, uint8_t(fill));  // edge chunks are padded with the fill value
+        const int64_t c0 = k * chunk, w = std::min<int64_t>(chunk, cols - c0);
+        for (int32_t r = 0; r < rows; ++r) memcpy(buf.data() + size_t(r) * size_t(chunk), window + r * pitch + c0, size_t(w));
+        uLongf len = uLongf(chunk_cap);
+        rc[size_t(k)] = compress2(out + k * chunk_cap, &len, buf.data(), uLong(raw), level);
+        sizes[k] = int64_t(len);
+    });
+    for (int64_t k = 0; k < n; ++k)
+        if (rc[size_t(k)] != Z_OK) return set_error(RSB_E_INVALID, "tiff_encode_chunks: compress2 of chunk %lld failed (%d)", (long long)k, rc[size_t(k)]);
     return RSB_OK;
 }

@@ -6,6 +6,9 @@
 in EPSG:3857, EPSG:4326 or a WGS 84 UTM zone (EPSG:32601-32660, 32701-32760). Anything else raises `RsbError` naming the value
 found. Overviews and sub-IFDs are ignored. `read_window` decodes a window of rows and columns with the library's decoder
 (`rsb_tiff_decode_window`) over a memory map of the file.
+
+`read_grid(path)` reads only the size and the georeferencing, with the same rules and messages for those, so any pixel layout
+(16-bit, JPEG, palette ...) is accepted: `rs mosaic --like` takes the grid of an existing raster.
 """
 
 import math
@@ -43,11 +46,9 @@ def _fail(path, what):
     raise _lib.RsbError("%s: %s" % (path, what))
 
 
-class GeoTiff:
-    """IFD 0 of a GeoTIFF. Attributes: width, height, spp (1, 3 or 4), alpha (the 4th sample is alpha), nodata (-1, or the 0..255
-    value of GDAL_NODATA), compression, predictor, tiled, chunk_w, chunk_h, offsets / byte_counts (int64 chunk table), epsg, crs
-    (see `crs_of_epsg`) and geotransform (c, a, b, f, d, e): X = c + a u + b v, Y = f + d u + e v for raster coordinates (u, v),
-    pixel (i, j) covering [i, i + 1) x [j, j + 1) (PixelIsPoint tiepoints are shifted by half a pixel, as GDAL does)."""
+class _Header:
+    """IFD 0's tags, its size (width, height) and its georeferencing (epsg, crs, geotransform, as `GeoTiff`); the pixel layout
+    is not looked at"""
 
     def __init__(self, path):
         self.path = path
@@ -57,6 +58,11 @@ class GeoTiff:
         self.file_len = size
         self._map = None
         self._parse()
+
+    def _parse(self):
+        self._parse_tags()
+        self._size()
+        self._georeference()
 
     # ---- container ----
 
@@ -68,7 +74,7 @@ class GeoTiff:
             _fail(self.path, "truncated file: %d bytes at offset %d are past its end (%d bytes)" % (n, offset, self.file_len))
         return b
 
-    def _parse(self):
+    def _parse_tags(self):
         head = self._data
         if len(head) < 8 or head[:2] not in (b"II", b"MM"):
             _fail(self.path, "not a TIFF file (first bytes %r)" % head[:4])
@@ -110,76 +116,18 @@ class GeoTiff:
                     vals = tuple(vals[i] / vals[i + 1] if vals[i + 1] else float("nan") for i in range(0, len(vals), 2))
                 tags[tag] = vals
         self._tags = tags
-        self._image()
-        self._georeference()
 
     def _tag(self, tag, default=None):
         v = self._tags.get(tag)
         return default if v is None else v
 
-    def _image(self):
+    def _size(self):
         t = self._tag
         if 256 not in self._tags or 257 not in self._tags:
             _fail(self.path, "no ImageWidth / ImageLength")
         self.width, self.height = int(t(256)[0]), int(t(257)[0])
         if self.width < 1 or self.height < 1:
             _fail(self.path, "empty image (%d x %d)" % (self.width, self.height))
-        self.compression = int(t(259, (1,))[0])
-        if self.compression not in COMPRESSIONS:
-            _fail(self.path, "Compression %d (%s) is not supported; use none, LZW or deflate" % (
-                self.compression, COMPRESSION_NAMES.get(self.compression, "unknown")))
-        self.spp = int(t(277, (1,))[0])
-        planar = int(t(284, (1,))[0])
-        if planar != 1:
-            _fail(self.path, "PlanarConfiguration %d is not supported; only 1 (chunky) is" % planar)
-        bits = t(258, (1,) * self.spp)
-        if any(int(b) != 8 for b in bits):
-            _fail(self.path, "BitsPerSample %s is not supported; only 8 is" % (",".join(str(int(b)) for b in bits)))
-        fmt = t(339, (1,) * self.spp)
-        if any(int(f) != 1 for f in fmt):
-            _fail(self.path, "SampleFormat %s is not supported; only 1 (unsigned integer) is" % (",".join(str(int(f)) for f in fmt)))
-        photometric = int(t(262, (1 if self.spp == 1 else 2,))[0])
-        extra = tuple(int(v) for v in t(338, ()))
-        if self.spp == 1 and photometric != 1:
-            _fail(self.path, "one band with Photometric %d (%s) is not supported; only MinIsBlack is" % (photometric, PHOTOMETRIC_NAMES.get(photometric, "unknown")))
-        if self.spp in (3, 4) and photometric != 2:
-            _fail(self.path, "%d bands with Photometric %d (%s) are not supported; only RGB is" % (self.spp, photometric, PHOTOMETRIC_NAMES.get(photometric, "unknown")))
-        if self.spp == 4 and extra not in ((1,), (2,)):
-            _fail(self.path, "4 bands with ExtraSamples %s are not supported; the 4th band must be alpha (1 or 2)" % (extra,))
-        if self.spp not in (1, 3, 4):
-            _fail(self.path, "%d bands are not supported; use 1 (gray), 3 (RGB) or 4 (RGB + alpha)" % self.spp)
-        self.alpha = self.spp == 4
-        self.predictor = int(t(317, (1,))[0])
-        if self.predictor not in (1, 2):
-            _fail(self.path, "Predictor %d is not supported; use 1 or 2" % self.predictor)
-        if self.compression == 1:
-            self.predictor = 1  # libtiff applies the predictor only inside a codec; uncompressed data is stored as is
-        if 322 in self._tags:
-            self.tiled = True
-            self.chunk_w, self.chunk_h = int(t(322)[0]), int(t(323, (0,))[0])
-            offsets, counts = t(324), t(325)
-            need = -(-self.width // max(1, self.chunk_w)) * -(-self.height // max(1, self.chunk_h))
-        else:
-            self.tiled = False
-            self.chunk_w, self.chunk_h = self.width, min(self.height, int(t(278, (2 ** 32 - 1,))[0]))
-            offsets, counts = t(273), t(279)
-            need = -(-self.height // max(1, self.chunk_h))
-        if self.chunk_w < 1 or self.chunk_h < 1:
-            _fail(self.path, "chunks of %d x %d pixels" % (self.chunk_w, self.chunk_h))
-        if offsets is None or counts is None or len(offsets) != need or len(counts) != need:
-            _fail(self.path, "%s table has %s offsets and %s byte counts, the image needs %d" % (
-                "tile" if self.tiled else "strip", None if offsets is None else len(offsets), None if counts is None else len(counts), need))
-        self.offsets = np.asarray(offsets, np.int64)
-        self.byte_counts = np.asarray(counts, np.int64)
-        nodata = self._tags.get(42113)
-        self.nodata = -1
-        if nodata:
-            try:
-                value = float(nodata.strip())
-            except ValueError:
-                _fail(self.path, "GDAL_NODATA %r is not a number" % nodata)
-            if math.isfinite(value) and value == int(value) and 0 <= value <= 255:  # any other value matches no 8-bit pixel
-                self.nodata = int(value)
 
     # ---- georeferencing ----
 
@@ -245,6 +193,78 @@ class GeoTiff:
             _fail(self.path, "degenerate geotransform %r" % ((c, a, b, f, d, e),))
         self.geotransform = (float(c), float(a), float(b), float(f), float(d), float(e))
 
+
+class GeoTiff(_Header):
+    """IFD 0 of a GeoTIFF. Attributes: width, height, spp (1, 3 or 4), alpha (the 4th sample is alpha), nodata (-1, or the 0..255
+    value of GDAL_NODATA), compression, predictor, tiled, chunk_w, chunk_h, offsets / byte_counts (int64 chunk table), epsg, crs
+    (see `crs_of_epsg`) and geotransform (c, a, b, f, d, e): X = c + a u + b v, Y = f + d u + e v for raster coordinates (u, v),
+    pixel (i, j) covering [i, i + 1) x [j, j + 1) (PixelIsPoint tiepoints are shifted by half a pixel, as GDAL does)."""
+
+    def _parse(self):
+        self._parse_tags()
+        self._size()
+        self._image()
+        self._georeference()
+
+    def _image(self):
+        t = self._tag
+        self.compression = int(t(259, (1,))[0])
+        if self.compression not in COMPRESSIONS:
+            _fail(self.path, "Compression %d (%s) is not supported; use none, LZW or deflate" % (
+                self.compression, COMPRESSION_NAMES.get(self.compression, "unknown")))
+        self.spp = int(t(277, (1,))[0])
+        planar = int(t(284, (1,))[0])
+        if planar != 1:
+            _fail(self.path, "PlanarConfiguration %d is not supported; only 1 (chunky) is" % planar)
+        bits = t(258, (1,) * self.spp)
+        if any(int(b) != 8 for b in bits):
+            _fail(self.path, "BitsPerSample %s is not supported; only 8 is" % (",".join(str(int(b)) for b in bits)))
+        fmt = t(339, (1,) * self.spp)
+        if any(int(f) != 1 for f in fmt):
+            _fail(self.path, "SampleFormat %s is not supported; only 1 (unsigned integer) is" % (",".join(str(int(f)) for f in fmt)))
+        photometric = int(t(262, (1 if self.spp == 1 else 2,))[0])
+        extra = tuple(int(v) for v in t(338, ()))
+        if self.spp == 1 and photometric != 1:
+            _fail(self.path, "one band with Photometric %d (%s) is not supported; only MinIsBlack is" % (photometric, PHOTOMETRIC_NAMES.get(photometric, "unknown")))
+        if self.spp in (3, 4) and photometric != 2:
+            _fail(self.path, "%d bands with Photometric %d (%s) are not supported; only RGB is" % (self.spp, photometric, PHOTOMETRIC_NAMES.get(photometric, "unknown")))
+        if self.spp == 4 and extra not in ((1,), (2,)):
+            _fail(self.path, "4 bands with ExtraSamples %s are not supported; the 4th band must be alpha (1 or 2)" % (extra,))
+        if self.spp not in (1, 3, 4):
+            _fail(self.path, "%d bands are not supported; use 1 (gray), 3 (RGB) or 4 (RGB + alpha)" % self.spp)
+        self.alpha = self.spp == 4
+        self.predictor = int(t(317, (1,))[0])
+        if self.predictor not in (1, 2):
+            _fail(self.path, "Predictor %d is not supported; use 1 or 2" % self.predictor)
+        if self.compression == 1:
+            self.predictor = 1  # libtiff applies the predictor only inside a codec; uncompressed data is stored as is
+        if 322 in self._tags:
+            self.tiled = True
+            self.chunk_w, self.chunk_h = int(t(322)[0]), int(t(323, (0,))[0])
+            offsets, counts = t(324), t(325)
+            need = -(-self.width // max(1, self.chunk_w)) * -(-self.height // max(1, self.chunk_h))
+        else:
+            self.tiled = False
+            self.chunk_w, self.chunk_h = self.width, min(self.height, int(t(278, (2 ** 32 - 1,))[0]))
+            offsets, counts = t(273), t(279)
+            need = -(-self.height // max(1, self.chunk_h))
+        if self.chunk_w < 1 or self.chunk_h < 1:
+            _fail(self.path, "chunks of %d x %d pixels" % (self.chunk_w, self.chunk_h))
+        if offsets is None or counts is None or len(offsets) != need or len(counts) != need:
+            _fail(self.path, "%s table has %s offsets and %s byte counts, the image needs %d" % (
+                "tile" if self.tiled else "strip", None if offsets is None else len(offsets), None if counts is None else len(counts), need))
+        self.offsets = np.asarray(offsets, np.int64)
+        self.byte_counts = np.asarray(counts, np.int64)
+        nodata = self._tags.get(42113)
+        self.nodata = -1
+        if nodata:
+            try:
+                value = float(nodata.strip())
+            except ValueError:
+                _fail(self.path, "GDAL_NODATA %r is not a number" % nodata)
+            if math.isfinite(value) and value == int(value) and 0 <= value <= 255:  # any other value matches no 8-bit pixel
+                self.nodata = int(value)
+
     # ---- pixels ----
 
     def read_window(self, row0, rows, col0, cols, out=None, threads=None):
@@ -269,3 +289,10 @@ class GeoTiff:
                                                        self.spp, self.compression, self.predictor, row0, rows, col0, cols, view.ctypes.data,
                                                        threads or usable_cores(), ctypes.byref(bad)), "%s" % self.path)
         return view.reshape(rows, cols, self.spp)
+
+
+def read_grid(path):
+    """(width, height, crs, geotransform) of the first image of a GeoTIFF, from its header alone: the size and the georeferencing
+    must be ones `GeoTiff` accepts (RsbError names the value found otherwise), the pixel layout may be anything."""
+    h = _Header(path)
+    return h.width, h.height, h.crs, h.geotransform

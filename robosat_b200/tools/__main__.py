@@ -1,9 +1,9 @@
-"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe,merge,extract,compare,tile} ...` --
+"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe,merge,extract,compare,tile,mosaic} ...` --
 the `rs` sub-commands on the hot path (dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
 
 import argparse
 
-from robosat_b200.tools import compare, cover, dedupe, extract, features, masks, merge, predict, rasterize, serve, tile, train, weights
+from robosat_b200.tools import compare, cover, dedupe, extract, features, masks, merge, mosaic, predict, rasterize, serve, tile, train, weights
 
 
 def add_parsers():
@@ -22,6 +22,7 @@ def add_parsers():
     extract.add_parser(subparser)
     compare.add_parser(subparser)
     tile.add_parser(subparser)
+    mosaic.add_parser(subparser)
     subparser.required = True
     return parser.parse_args()
 
