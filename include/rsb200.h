@@ -306,6 +306,37 @@ int rsb_label_components(const uint8_t* planes, int64_t image_stride, int32_t N,
 int rsb_building_clean(const uint8_t* opened, int64_t image_stride, int32_t N, int32_t H, int32_t W, int32_t min_area, int32_t min_hole_area,
                        int32_t* labels, int32_t* stats, uint8_t* out, int32_t* fg_counts, void* stream);
 
+/* `rs features --type road` (the rule is DESIGN.md §8): thinning, m-degrees, spur pruning and chain lists of N halo'd planes of
+ * H x W. 1 <= N <= 65535, 1 <= H, W <= RSB_ROAD_MAX_SIZE; every output is laid out [N][H][W] (contiguous). Pixel indices are
+ * plane-local, y * W + x. Arguments are validated before the device check; nothing allocates or synchronises.
+ *
+ * rsb_road_thin: Zhang-Suen (1984) of (plane != 0), image n at planes + n * image_stride, pixels outside the plane background,
+ * until the first full iteration that deletes nothing -> skel uint8 {0, 1}, iterations int32 [N] (full iterations run, the last
+ * one included). One CTA per plane keeps it bit-packed in shared memory, so H * ceil(W / 32) <= RSB_ROAD_MAX_WORDS (a 640 x 640
+ * plane takes 12 800 words); a larger plane is refused with RSB_E_UNSUPPORTED.
+ * rsb_road_degree: deg int8 = the m-degree of each pixel of skel (4-neighbours, and diagonal neighbours with no common
+ * 4-neighbour in skel), -1 off skel.
+ * rsb_road_prune: out = skel without every chain of (skel, deg) that runs from an endpoint to a junction (degree >= 3) with fewer
+ * than min_length pixels not counting the junction, or from an endpoint to an endpoint with fewer than min_length pixels.
+ * rsb_road_chain_count: with deg the degrees of skel and labels / flags the labels / areas rsb_label_components gives for
+ * (skel == 1) under 8-connectivity (flags is overwritten): counts int32 [N][H][W] per pixel (workspace), row_offsets int64
+ * [N][H] (workspace), totals int64 [N] = each plane's (chain count << 32 | pixel count of its lists).
+ * rsb_road_chain_write: the same skel, deg, labels, flags, counts and row_offsets; chain_base / pixel_base int64 [N] the index of
+ * plane n's first chain and first pixel in the outputs (prefix sums of totals) -> chain_offsets int64 [chains] the start of each
+ * chain in pixels, pixels int32 the chains' pixel indices. A plane's chains come in (first pixel, second pixel) order; each is
+ * written from its end with the smaller index (a loop at one node, or a node-free cycle from its smallest pixel, toward the
+ * smaller second pixel, repeating the first pixel at the end). */
+#define RSB_ROAD_MAX_SIZE 4096
+#define RSB_ROAD_MAX_WORDS 16384
+int rsb_road_thin(const uint8_t* planes, int64_t image_stride, int32_t N, int32_t H, int32_t W, uint8_t* skel, int32_t* iterations, void* stream);
+int rsb_road_degree(const uint8_t* skel, int32_t N, int32_t H, int32_t W, int8_t* deg, void* stream);
+int rsb_road_prune(const uint8_t* skel, const int8_t* deg, int32_t N, int32_t H, int32_t W, int32_t min_length, uint8_t* out, void* stream);
+int rsb_road_chain_count(const uint8_t* skel, const int8_t* deg, const int32_t* labels, int32_t* flags, int32_t N, int32_t H, int32_t W,
+                         int32_t* counts, int64_t* row_offsets, int64_t* totals, void* stream);
+int rsb_road_chain_write(const uint8_t* skel, const int8_t* deg, const int32_t* labels, const int32_t* flags, int32_t N, int32_t H, int32_t W,
+                         const int32_t* counts, const int64_t* row_offsets, const int64_t* chain_base, const int64_t* pixel_base,
+                         int64_t* chain_offsets, int32_t* pixels, void* stream);
+
 /* `rs rasterize` polygon fill (robosat/tools/rasterize.py:64-83: rasterio.features.rasterize, all_touched=False, burn value 1,
  * merge "replace"). All arrays are DEVICE pointers. Polygons: vertices float64 [num_vertices][2] (EPSG:3857 X, Y; 16-byte aligned);
  * ring r owns vertices [ring_offsets[r], ring_offsets[r + 1]) and is closed implicitly; polygon p owns rings

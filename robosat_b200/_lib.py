@@ -83,6 +83,8 @@ class ConvDesc(ctypes.Structure):
 RSB_MORPH_MAX_OPS = 4
 RSB_MORPH_MAX_K = 64
 RSB_LABEL_MAX_SIZE = 8192
+RSB_ROAD_MAX_SIZE = 4096
+RSB_ROAD_MAX_WORDS = 16384
 RSB_RASTER_MAX_SIZE = 4096
 RSB_COVER_MAX_WIDTH = 1856000
 RSB_COVER_MAX_ZOOM = 30
@@ -207,6 +209,11 @@ SIGNATURES = {
     "rsb_morph_binary": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, ctypes.POINTER(MorphOp), _i32, _vp, _vp, _vp]),
     "rsb_label_components": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "rsb_building_clean": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "rsb_road_thin": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "rsb_road_degree": (ctypes.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
+    "rsb_road_prune": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "rsb_road_chain_count": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "rsb_road_chain_write": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rsb_rasterize_polygons": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]),
     "rsb_cover_polygons": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _vp, _vp]),
     "rsb_cover_emit_keys": (ctypes.c_int, [_vp, _i64, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]),

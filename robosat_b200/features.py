@@ -478,3 +478,210 @@ class BuildingHandler(ParkingHandler):
         work = [(tiles[i], m) for i, m in zip(full, masks)]
         run = lambda tm: polygons_from_filled(tm[0], tm[1], self.simplify_epsilon)  # noqa: E731
         self._gather(pool.map(run, work) if pool is not None else map(run, work))
+
+
+# --- roads (this project's rule; the reference has no road handler: DESIGN.md §8) ------------------------------------------------
+
+def road_thin_device(planes):
+    """planes: uint8 CUDA tensor [N, H, W] (rows contiguous) -> (uint8 [N, H, W] {0, 1} Zhang-Suen skeleton of (planes != 0), int32
+    [N] full iterations run, the last one that deleted nothing included). Refuses a plane of more than RSB_ROAD_MAX_WORDS 32-bit
+    row words with an RsbError before any launch. Enqueued on the current stream, no synchronisation."""
+    import torch
+
+    N, H, W, stride = _planes(planes, "road_thin_device")
+    skel = torch.empty((N, H, W), dtype=torch.uint8, device=planes.device)
+    iterations = torch.empty((N,), dtype=torch.int32, device=planes.device)
+    _lib.check(_lib.load().rsb_road_thin(planes.data_ptr(), stride, N, H, W, skel.data_ptr(), iterations.data_ptr(), _lib.current_stream_ptr()),
+               "rsb_road_thin")
+    return skel, iterations
+
+
+def _contiguous(t, dtype, what):
+    import torch
+
+    if not t.is_cuda or t.dtype != getattr(torch, dtype) or t.dim() != 3 or not t.is_contiguous():
+        raise ValueError("%s needs a contiguous %s CUDA tensor [N, H, W]" % (what, dtype))
+    return t.shape
+
+
+def road_degree_device(skel):
+    """skel: contiguous uint8 CUDA tensor [N, H, W] {0, 1} -> int8 [N, H, W] m-degree of every skeleton pixel, -1 off it"""
+    import torch
+
+    N, H, W = _contiguous(skel, "uint8", "road_degree_device")
+    deg = torch.empty((N, H, W), dtype=torch.int8, device=skel.device)
+    _lib.check(_lib.load().rsb_road_degree(skel.data_ptr(), N, H, W, deg.data_ptr(), _lib.current_stream_ptr()), "rsb_road_degree")
+    return deg
+
+
+def road_prune_device(skel, deg, min_length):
+    """skel, deg: contiguous [N, H, W] from road_thin_device / road_degree_device -> uint8 [N, H, W] skel without its spurs and
+    short isolated pieces (fewer than min_length pixels, a spur's junction not counted), decided in one pass on (skel, deg)"""
+    import torch
+
+    N, H, W = _contiguous(skel, "uint8", "road_prune_device")
+    if _contiguous(deg, "int8", "road_prune_device") != skel.shape:
+        raise ValueError("road_prune_device: deg and skel differ in shape")
+    out = torch.empty_like(skel)
+    _lib.check(_lib.load().rsb_road_prune(skel.data_ptr(), deg.data_ptr(), N, H, W, int(min_length), out.data_ptr(), _lib.current_stream_ptr()),
+               "rsb_road_prune")
+    return out
+
+
+def road_chains_device(skel, deg):
+    """skel, deg: contiguous [N, H, W] -> per plane a list of int32 arrays, the pixel indices y * W + x of each chain of the graph
+    (DESIGN.md §8), in (first pixel, second pixel) order. Synchronises once for the per-plane totals; planes without chains copy
+    nothing back."""
+    import torch
+
+    from robosat_b200.cover import _alloc
+
+    N, H, W = _contiguous(skel, "uint8", "road_chains_device")
+    if _contiguous(deg, "int8", "road_chains_device") != skel.shape:
+        raise ValueError("road_chains_device: deg and skel differ in shape")
+    dev = skel.device
+    lib, stream = _lib.load(), _lib.current_stream_ptr()
+    labels, flags = components_device(skel, 1, 8)
+    counts = _alloc((N, H, W), torch.int32, dev, "road chain counts")
+    rows = torch.empty((N, H), dtype=torch.int64, device=dev)
+    totals = torch.empty((N,), dtype=torch.int64, device=dev)
+    _lib.check(lib.rsb_road_chain_count(skel.data_ptr(), deg.data_ptr(), labels.data_ptr(), flags.data_ptr(), N, H, W, counts.data_ptr(),
+                                        rows.data_ptr(), totals.data_ptr(), stream), "rsb_road_chain_count")
+    t = totals.cpu().numpy()
+    nchains, npixels = (t >> 32).astype(np.int64), (t & 0xffffffff).astype(np.int64)
+    out = [[] for _ in range(N)]
+    if nchains.sum() == 0:
+        return out
+    chain_base = np.concatenate([[0], np.cumsum(nchains)[:-1]])
+    pixel_base = np.concatenate([[0], np.cumsum(npixels)[:-1]])
+    offsets = _alloc((int(nchains.sum()),), torch.int64, dev, "road chain offsets")
+    pixels = _alloc((int(npixels.sum()),), torch.int32, dev, "road chain pixels")
+    cb, pb = torch.from_numpy(chain_base).to(dev), torch.from_numpy(pixel_base).to(dev)
+    _lib.check(lib.rsb_road_chain_write(skel.data_ptr(), deg.data_ptr(), labels.data_ptr(), flags.data_ptr(), N, H, W, counts.data_ptr(),
+                                        rows.data_ptr(), cb.data_ptr(), pb.data_ptr(), offsets.data_ptr(), pixels.data_ptr(), stream),
+               "rsb_road_chain_write")
+    offsets, pixels = offsets.cpu().numpy(), pixels.cpu().numpy()
+    ends = np.append(offsets[1:], len(pixels))
+    for n in np.flatnonzero(nchains):
+        c0, c1 = chain_base[n], chain_base[n] + nchains[n]
+        out[n] = [pixels[offsets[c]:ends[c]] for c in range(c0, c1)]
+    return out
+
+
+def road_device(planes, min_area=256, min_hole_area=256, min_length=20):
+    """planes: uint8 CUDA tensor [N, H, W] of halo'd binary road masks {0, 1} -> per plane the list of its chains (int32 pixel
+    indices y * W + x of the plane): the cleanup (`rsb_building_clean`), the thinning, the spur pruning and the chains of what
+    remains (DESIGN.md §8). Synchronises once."""
+    import torch
+
+    from robosat_b200.cover import _alloc
+
+    N, H, W, stride = _planes(planes, "road_device")
+    work = _alloc((N, H, W), torch.int32, planes.device, "road component labels")
+    stats = _alloc((N, H, W), torch.int32, planes.device, "road component areas")
+    clean = torch.empty((N, H, W), dtype=torch.uint8, device=planes.device)
+    counts = torch.empty((N,), dtype=torch.int32, device=planes.device)
+    _lib.check(_lib.load().rsb_building_clean(planes.data_ptr(), stride, N, H, W, int(min_area), int(min_hole_area), work.data_ptr(),
+                                              stats.data_ptr(), clean.data_ptr(), counts.data_ptr(), _lib.current_stream_ptr()),
+               "rsb_building_clean")
+    del work, stats
+    skel, _ = road_thin_device(clean)
+    pruned = road_prune_device(skel, road_degree_device(skel), min_length)
+    return road_chains_device(pruned, road_degree_device(pruned))
+
+
+def halo_plane(center, neighbours, class_index, halo, out):
+    """Writes the halo'd binary plane of one tile into out (uint8 [H + 2 halo, W + 2 halo]): (mask == class_index) of the tile and
+    of the halo-px strips of its 8 neighbours; `neighbours[(dy, dx)]` is a neighbour's mask or None (background)."""
+    H, W = center.shape
+    h = halo
+    out[:] = 0
+    for dy in (-1, 0, 1):
+        for dx in (-1, 0, 1):
+            m = center if (dy, dx) == (0, 0) else neighbours.get((dy, dx))
+            if m is None:
+                continue
+            ys = slice(H - h, H) if dy < 0 else (slice(0, h) if dy > 0 else slice(0, H))
+            xs = slice(W - h, W) if dx < 0 else (slice(0, h) if dx > 0 else slice(0, W))
+            oy = 0 if dy < 0 else (h + H if dy > 0 else h)
+            ox = 0 if dx < 0 else (h + W if dx > 0 else h)
+            sub = m[ys, xs]
+            np.equal(sub, class_index, out=out[oy:oy + sub.shape[0], ox:ox + sub.shape[1]].view(bool))
+
+
+def _runs(chain, H, W, halo):
+    """The maximal runs of a chain's pixels inside the tile -> [(points [(x, y)], closed)] in tile pixel coordinates: pixel centres,
+    plus the midpoint of the two centres where a run continues to a pixel outside the tile"""
+    Wp = W + 2 * halo
+    y, x = chain // Wp - halo, chain % Wp - halo
+    inside = (y >= 0) & (y < H) & (x >= 0) & (x < W)
+    if not inside.any():
+        return []
+    cx, cy = x + 0.5, y + 0.5
+    if inside.all() and chain[0] == chain[-1]:
+        return [([(float(a), float(b)) for a, b in zip(cx[:-1], cy[:-1])], True)]
+    out = []
+    edges = np.flatnonzero(np.diff(np.concatenate([[0], inside.astype(np.int8), [0]])))
+    for i, j in zip(edges[0::2], edges[1::2]):
+        pts = [(float(a), float(b)) for a, b in zip(cx[i:j], cy[i:j])]
+        if i > 0:
+            pts.insert(0, (0.5 * float(cx[i - 1] + cx[i]), 0.5 * float(cy[i - 1] + cy[i])))
+        if j < len(chain):
+            pts.append((0.5 * float(cx[j - 1] + cx[j]), 0.5 * float(cy[j - 1] + cy[j])))
+        if len(pts) >= 2:
+            out.append((pts, False))
+    return out
+
+
+def lines_from_chains(tile, chains, shape, halo, simplify_epsilon=1.0):
+    """Host half of `RoadHandler`: the chains of one halo'd plane (pixel indices of the plane) -> LineString features of the tile
+    of `shape` (rows, cols): each chain cut into its runs inside the tile, simplified with `approxPolyDP(epsilon)` (closed for a
+    whole cycle inside the tile, which then repeats its first point) and mapped to lon/lat. Thread-safe."""
+    import cv2
+
+    H, W = shape
+    features = []
+    for chain in chains:
+        for pts, closed in _runs(np.asarray(chain, dtype=np.int64), H, W, halo):
+            simple = cv2.approxPolyDP(np.array(pts, dtype=np.float32).reshape(-1, 1, 2), simplify_epsilon, closed).reshape(-1, 2)
+            line = [(float(a), float(b)) for a, b in simple]
+            if closed:
+                line.append(line[0])
+            if len(line) < 2:
+                continue
+            coords = [list(pixel_to_location(tile, a / W, 1. - b / H)) for a, b in line]
+            features.append({"type": "Feature", "geometry": {"type": "LineString", "coordinates": coords}, "properties": {}})
+    return features
+
+
+class RoadHandler(ParkingHandler):
+    """Road centre lines: `apply_batch` for a batch of halo'd binary road planes on the device, `save(out)`.
+
+    The cleanup, the thinning, the spur pruning and the chains run on the device (`road_device`); the crop to the tile, the
+    simplification and the transform to lon/lat run on the host in `lines_from_chains`. The thresholds are this project's choices
+    for z18 tiles (DESIGN.md §8), not tuned against imagery."""
+
+    halo = 64
+    min_area = 256
+    min_hole_area = 256
+    min_length = 20
+    simplify_epsilon = 1.0
+
+    def check_zoom(self, tile):
+        if tile.z != 18:
+            raise NotImplementedError("Road post-processing thresholds are set for z18")
+
+    def apply(self, tile, mask):
+        raise NotImplementedError("roads need each tile's neighbours: use apply_batch with halo'd planes (rs features --type road)")
+
+    def apply_batch(self, tiles, planes_device, pool=None):
+        """tiles: N tiles; planes_device: uint8 CUDA tensor [N, H + 2 halo, W + 2 halo] of halo'd binary road planes (`halo_plane`).
+        Features are appended in tile order. Planes without chains do no host work. `pool` (an Executor) runs the host step."""
+        for t in tiles:
+            self.check_zoom(t)
+        chains = road_device(planes_device, self.min_area, self.min_hole_area, self.min_length)
+        _, Hp, Wp = planes_device.shape
+        shape = (Hp - 2 * self.halo, Wp - 2 * self.halo)
+        work = [(tiles[i], c) for i, c in enumerate(chains) if c]
+        run = lambda tc: (lines_from_chains(tc[0], tc[1], shape, self.halo, self.simplify_epsilon), [])  # noqa: E731
+        self._gather(pool.map(run, work) if pool is not None else map(run, work))
