@@ -183,6 +183,19 @@ class TilePredictor:
         slot["busy"] = True
         self._pending.append(slot)
 
+    def submit_resident(self):
+        """`submit_device` that leaves the bins on the device: forward and head only, no device-to-host copy. Returns the slot's
+        device bins, which work enqueued on the current stream may read until `depth` more submits."""
+        slot = self._slots[self._next % self.depth]
+        self._next += 1
+        main = torch.cuda.current_stream(self.device)
+        if slot.get("busy"):
+            main.wait_event(slot["done"])  # an earlier submit's device-to-host copy has read the bins this one overwrites
+        self._compute(slot)
+        slot["consumed"].record(main)
+        slot["computed"].record(main)
+        return slot["d_q"]
+
     def pinned_input(self):
         """The pinned staging buffer the next `submit` will use (fill it in place to skip one host copy)."""
         return self._slots[self._next % self.depth]["h_in"]

@@ -1,9 +1,9 @@
-"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe,merge,extract,compare,tile,mosaic} ...` --
+"""`python -m robosat_b200.tools {train,predict,serve,masks,weights,features,rasterize,cover,dedupe,merge,extract,compare,tile,mosaic,segment} ...` --
 the `rs` sub-commands on the hot path (dispatch as in robosat/tools/__main__.py:22-59; the other sub-commands stay with the reference package)."""
 
 import argparse
 
-from robosat_b200.tools import compare, cover, dedupe, extract, features, masks, merge, mosaic, predict, rasterize, serve, tile, train, weights
+from robosat_b200.tools import compare, cover, dedupe, extract, features, masks, merge, mosaic, predict, rasterize, segment, serve, tile, train, weights
 
 
 def add_parsers():
@@ -23,6 +23,7 @@ def add_parsers():
     compare.add_parser(subparser)
     tile.add_parser(subparser)
     mosaic.add_parser(subparser)
+    segment.add_parser(subparser)
     subparser.required = True
     return parser.parse_args()
 

@@ -324,6 +324,11 @@ def run_shard(rank, world, args, device, sd, num_classes, stats=None):
     return st
 
 
+def load_state_dict(path):
+    # https://github.com/pytorch/pytorch/issues/7178 -- always deserialise to host memory first
+    return torch.load(path, map_location="cpu")["state_dict"]
+
+
 def _run(rank, world, args, port):
     from robosat_b200.dist import broadcast_state_dict, check_async_error, unet_state_template
 
@@ -332,10 +337,7 @@ def _run(rank, world, args, port):
     torch.cuda.set_device(rank)
     device = torch.device("cuda", rank)
 
-    sd = None
-    if rank == 0:
-        # https://github.com/pytorch/pytorch/issues/7178 -- always deserialise to host memory first
-        sd = torch.load(args.checkpoint, map_location="cpu")["state_dict"]
+    sd = load_state_dict(args.checkpoint) if rank == 0 else None
     if world > 1:
         import torch.distributed as dist
 
