@@ -652,6 +652,20 @@ int rsb_tile_warp(const uint8_t* src, int64_t src_pitch, int64_t win_row0, int64
                   int64_t node_y0, int32_t nodes_w, int32_t nodes_h, int32_t grid_step, const int64_t* tiles, int32_t N, int32_t size,
                   int32_t resampling, uint8_t* out, int64_t image_stride, int64_t* covered, int64_t* misses, void* stream);
 
+/* `rs tile --resampling average` (DESIGN.md §8): the arguments of rsb_tile_warp without `resampling`, but nodes hold the source
+ * coordinates (u, v) of global tile pixel corners (kG, lG). Each corner of pixel (gx, gy), the integer corners (gx, gy) to
+ * (gx + 1, gy + 1), interpolates the four nodes of the lattice cell that contains it; the pixel averages the source pixels its corners'
+ * axis-aligned bounding box overlaps, clipped to the raster, weighted by the overlap of each pixel's row and column with the box and
+ * summed row by row over valid pixels, every float64 operation rounded separately. A pixel with a NaN corner, an empty clipped box
+ * or no valid weight is uncovered (0, 0, 0). A box wider or taller than RSB_TILE_MAX_FOOTPRINT source pixels is not summed: the pixel
+ * is uncovered and counted in misses (the host refuses such runs first). Arguments are validated before the device check; allocates
+ * nothing and does not synchronise. */
+#define RSB_TILE_MAX_FOOTPRINT 64
+int rsb_tile_average(const uint8_t* src, int64_t src_pitch, int64_t win_row0, int64_t win_col0, int64_t win_rows, int64_t win_cols,
+                     int64_t raster_w, int64_t raster_h, int32_t spp, int32_t alpha, int32_t nodata, const double* nodes, int64_t node_x0,
+                     int64_t node_y0, int32_t nodes_w, int32_t nodes_h, int32_t grid_step, const int64_t* tiles, int32_t N, int32_t size,
+                     uint8_t* out, int64_t image_stride, int64_t* covered, int64_t* misses, void* stream);
+
 /* rs mosaic (DESIGN.md §8): deflate the chunk x chunk tiles of one row of a 1-band 8-bit raster window. window_host uint8 rows x cols
  * (row pitch `pitch`, rows <= chunk); tile k holds columns [k chunk, (k + 1) chunk) and is padded with `fill` past the window's rows
  * and columns, then zlib-compressed (compress2 at `level`) into out_host + k * chunk_cap; sizes_host int64 [ceil(cols / chunk)] gets

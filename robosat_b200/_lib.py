@@ -106,6 +106,7 @@ RSB_COMPARE_MAX_PLANES = 32
 RSB_COMPARE_MAX_CLASSES = 256
 RSB_TILE_MAX_SIZE = 4096
 RSB_TILE_MAX_STEP = 64
+RSB_TILE_MAX_FOOTPRINT = 64
 
 
 class MorphOp(ctypes.Structure):
@@ -252,6 +253,8 @@ SIGNATURES = {
                                               _vp, _i32, _vp]),
     "rsb_tile_warp": (ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _vp, _i32,
                                      _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
+    "rsb_tile_average": (ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _vp,
+                                        _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
     "rsb_tiff_deflate_bound": (_i64, [_i64]),
     "rsb_tiff_encode_chunks": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i32]),
     "rsb_mosaic_warp": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _i64, _i64,

@@ -6,9 +6,10 @@ The rule is a composition and nothing else (DESIGN.md §8): the output's pixels 
     rs tile → rs predict → rs masks → rs mosaic --like ortho.tif
 
 run with the same settings. So the tiles are `tile.candidate_tiles` (intersected with `--tiles`) warped by `tile.plan`'s windows
-with `tile.choose_step`'s lattice, a tile exists when it has a covered pixel, each existing tile is predicted with the halo of its
-existing neighbours (black where a neighbour does not exist), the bins become masks with the soft vote of one model, and the
-output windows are `mosaic.plan`'s over the grid of the source raster, sampled nearest with missing tiles invalid.
+with `tile.choose_step`'s lattice (the corner lattice for `average`), a tile exists when it has a covered pixel, each existing
+tile is predicted with the halo of its existing neighbours (black where a neighbour does not exist), the bins become masks with
+the soft vote of one model, and the output windows are `mosaic.plan`'s over the grid of the source raster, sampled nearest with
+missing tiles invalid.
 
 Nothing is written to or read from disk between the steps. Two device stores hold what is in flight, both rings indexed by the
 warped tiles in row-major order (tile i lives in slot i mod slots):
@@ -44,6 +45,7 @@ class Plan:
     """The schedule of one run.
 
     tiles       int64 [n, 2], the warped tiles (x, y) in row-major order; tile i is index i
+    corner      whether the warps' lattice is the corner lattice of `average` (tile.plan's `corner`)
     warps       the tile.Window of `tile.plan`, in the same order; warp k writes indices [first[k], first[k + 1])
     neighbours  int64 [n, 9], the index of each tile's neighbour in `stitch.NEIGHBOURS` order, -1 when it is not warped
     batches     [(a, b)]: batch j predicts indices [a, b)
@@ -60,21 +62,25 @@ def _index_of(tiles):
     return {(int(x), int(y)): i for i, (x, y) in enumerate(tiles.tolist())}
 
 
-def plan(raster, grid, zoom, size, batch=DEFAULT_BATCH, tiles=None, budget=DEFAULT_BUDGET):
+def plan(raster, grid, zoom, size, batch=DEFAULT_BATCH, tiles=None, budget=DEFAULT_BUDGET, resampling="bilinear"):
     """The Plan of segmenting `raster` (a GeoTiff, or anything with width, height, spp, crs and geotransform) onto `grid` (a
     mosaic.Grid) with tiles of `size` pixels at `zoom` and batches of `batch`. `tiles` (iterable of (x, y)) restricts the candidate
-    tiles as `rs tile --tiles` does. Host only. RsbError, before anything is allocated, when the stores' peak exceeds `budget`."""
+    tiles as `rs tile --tiles` does; `resampling` is the image warp's, as in `rs tile`, and picks the lattice. Host only. RsbError,
+    before anything is allocated, when the stores' peak exceeds `budget` or (average) a footprint exceeds the cap of `tile.plan`."""
     if batch < 1:
         raise ValueError("batch must be at least 1")
+    if resampling not in T.RESAMPLINGS:
+        raise ValueError("resampling must be one of %s" % ", ".join(T.RESAMPLINGS))
     cand = T.candidate_tiles(raster, zoom, size)
     if tiles is not None:
         want = {(int(x), int(y)) for x, y in tiles}
         cand = cand[np.array([(int(x), int(y)) in want for x, y in cand], bool)] if len(cand) else cand
     p = Plan()
     p.zoom, p.size, p.batch, p.budget = zoom, size, batch, budget
+    p.corner = resampling == "average"
     p.candidates = len(cand)
-    p.step = T.choose_step(raster, zoom, size, cand)
-    p.warps = T.plan(raster, zoom, size, cand, p.step)
+    p.step = T.choose_step(raster, zoom, size, cand, p.corner)
+    p.warps = T.plan(raster, zoom, size, cand, p.step, corner=p.corner)
     p.tiles = np.array([(x, w.y) for w in p.warps for x in w.xs], np.int64).reshape(-1, 2)
     p.first = np.cumsum([0] + [len(w.xs) for w in p.warps]).astype(np.int64)
     n = len(p.tiles)
@@ -166,7 +172,7 @@ def output_palette(flat):
 
 def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, sink=None, device="cuda", stats=None, threads=None):
     """Execute Plan `p` on one device. `predictor`: a TilePredictor of p.batch tiles of p.size + 2 overlap pixels. `resampling`: the
-    image warp's, as in `rs tile`. output 'masks':
+    image warp's, as in `rs tile`, and must be the one `p` was planned for. output 'masks':
     the class of each pixel (the soft vote of one model); 'probs' (two classes only): the foreground bins. sink(window, pixels) is
     called on a writer thread for every output window, in schedule order, with pixels uint8 [rows, cols] (None: every pixel is
     nodata). Returns the number of existing tiles. `stats`, a dict, receives the counts and the seconds of decode, warp, predict
@@ -175,8 +181,10 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
 
     from robosat_b200.hostinfo import usable_cores
 
-    if resampling not in T.RESAMPLING:
-        raise ValueError("resampling must be one of %s" % ", ".join(T.RESAMPLING))
+    if resampling not in T.RESAMPLINGS:
+        raise ValueError("resampling must be one of %s" % ", ".join(T.RESAMPLINGS))
+    if (resampling == "average") != p.corner:
+        raise ValueError("the plan's lattice is for %s, not %s resampling" % ("average" if p.corner else "nearest or bilinear", resampling))
     if output not in OUTPUTS:
         raise ValueError("output must be one of %s" % ", ".join(OUTPUTS))
     C = predictor.classes
@@ -209,7 +217,6 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
         covered = torch.empty((nmax,), dtype=torch.int64, device=dev)
         misses = torch.zeros((2,), dtype=torch.int64, device=dev)
         counts_host = torch.empty((nmax + 2,), dtype=torch.int64, pin_memory=True)
-    mode = T.RESAMPLING[resampling]
     stitched = {}  # batch -> event recorded after its stitch (a later warp into the same image slots waits for it)
     timing = {"warp_s": [], "predict_s": [], "mosaic_s": []}
 
@@ -258,18 +265,16 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
             if parts[0][1] < b - a:  # the window wraps around the end of the ring: the rest goes to slot 0 on
                 parts.append((parts[0][1], b - a, 0))
             for q, (i0, i1, slot) in enumerate(parts):
-                _lib.check(lib.rsb_tile_warp(src.data_ptr(), w.cols * spp, w.row0, w.col0, w.rows, w.cols, raster.width, raster.height, spp,
-                                             int(raster.alpha), raster.nodata, nodes.data_ptr(), w.kx0, w.ky0, w.nodes.shape[1], w.nodes.shape[0],
-                                             p.step, xy[i0:].data_ptr(), i1 - i0, S, mode, images[slot].data_ptr(), image,
-                                             covered[i0:].data_ptr(), misses[q:].data_ptr(), _lib.current_stream_ptr()), "rsb_tile_warp")
+                T.warp(lib, resampling, src.data_ptr(), w, raster, nodes.data_ptr(), p.step, xy[i0:].data_ptr(), i1 - i0, S, images[slot].data_ptr(),
+                       image, covered[i0:].data_ptr(), misses[q:].data_ptr())
             end.record(side)
             counts_host[:b - a].copy_(covered[:b - a], non_blocking=True)
             counts_host[nmax:nmax + 2].copy_(misses, non_blocking=True)
         side.synchronize()  # the decode of window k + 2 reuses this window's pinned buffer; the counts decide what exists
         missed = int(counts_host[nmax]) + int(counts_host[nmax + 1])
         if missed:
-            raise _lib.RsbError("rsb_tile_warp: %d samples of tiles %d..%d of row %d fell outside their source window (a planning error)" % (
-                missed, w.xs[0], w.xs[-1], w.y))
+            raise _lib.RsbError("%s: %d samples of tiles %d..%d of row %d fell outside their source window (a planning error)" % (
+                T.entry_point(resampling), missed, w.xs[0], w.xs[-1], w.y))
         exists[a:b] = counts_host[:b - a].numpy() > 0
         return nxt
 

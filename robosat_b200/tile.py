@@ -16,6 +16,9 @@ restated in tests/tile_reference.py:
   are (0, 0, 0).
 - Candidate tiles are those whose Mercator box meets the raster footprint (the box of the raster boundary sampled at every edge
   pixel corner, widened by one tile pixel); a tile is produced only when it has a covered pixel.
+- Area averaging (`average`, `rsb_tile_average`) takes the lattice at pixel corners instead (`corner=True` below): each pixel
+  averages the source pixels under the bounding box of its four interpolated corners, weighted by their overlap with it. A footprint
+  may span at most RSB_TILE_MAX_FOOTPRINT source pixels; `plan` refuses a run that could exceed it.
 
 Work goes in windows: a run of at most `batch` adjacent tiles of one tile row, whose source rows and columns (from the lattice,
 plus 2 pixels) and output fit `budget` device bytes. The next window is decoded on a host thread while the current one is warped,
@@ -39,8 +42,10 @@ DEFAULT_BATCH = 64
 STEPS = (64, 32, 16, 8, 4, 2, 1)
 TOLERANCE = 0.125  # source pixels between the exact transform and the lattice interpolation at every cell centre
 MARGIN = 2  # source pixels added around a window's lattice range
-RESAMPLING = {"nearest": 0, "bilinear": 1}
-W_COARSE = "Warning: a zoom {} pixel spans {:.1f} raster pixels; bilinear resampling aliases above 2 (area averaging is not implemented)"
+RESAMPLING = {"nearest": 0, "bilinear": 1}  # the codes of rsb_tile_warp
+RESAMPLINGS = ("nearest", "bilinear", "average")  # average runs rsb_tile_average on the corner lattice
+W_COARSE = "Warning: a zoom {} pixel spans {:.1f} raster pixels; bilinear resampling aliases above 2 (use --resampling average)"
+FOOTPRINT_SLACK = 1e-6  # source pixels added to the host's bound of a footprint's extent, for the rounding of the interpolation
 
 
 # ---- projections (numpy float64, elementwise) ----
@@ -165,26 +170,32 @@ def source_coords(raster, X, Y):
     return c + a * mx + b * my, f + d * mx + e * my
 
 
-def pixel_centre(g, zoom, size):
-    """global pixel index -> Mercator coordinate of its centre along x (Y is its negation)"""
-    return -CE / 2 + (np.asarray(g, np.float64) + 0.5) * (CE / (2.0 ** zoom * size))
+def pixel_centre(g, zoom, size, corner=False):
+    """global pixel index -> Mercator coordinate of its centre (its left corner when `corner`) along x (Y is its negation)"""
+    g = np.asarray(g, np.float64)
+    return -CE / 2 + (g if corner else g + 0.5) * (CE / (2.0 ** zoom * size))
 
 
-def lattice(raster, zoom, size, step, kx0, kx1, ky0, ky1):
-    """float64 [ky1 - ky0 + 1, kx1 - kx0 + 1, 2]: (u, v) at the centres of global pixels (k step, l step), kx0 <= k <= kx1,
-    ky0 <= l <= ky1"""
-    X = pixel_centre(np.arange(kx0, kx1 + 1, dtype=np.int64) * step, zoom, size)
-    Y = -pixel_centre(np.arange(ky0, ky1 + 1, dtype=np.int64) * step, zoom, size)
+def lattice(raster, zoom, size, step, kx0, kx1, ky0, ky1, corner=False):
+    """float64 [ky1 - ky0 + 1, kx1 - kx0 + 1, 2]: (u, v) at the centres (the top-left corners when `corner`) of global pixels
+    (k step, l step), kx0 <= k <= kx1, ky0 <= l <= ky1"""
+    X = pixel_centre(np.arange(kx0, kx1 + 1, dtype=np.int64) * step, zoom, size, corner)
+    Y = -pixel_centre(np.arange(ky0, ky1 + 1, dtype=np.int64) * step, zoom, size, corner)
     u, v = source_coords(raster, *np.meshgrid(X, Y))
     return np.ascontiguousarray(np.stack([u, v], axis=-1))
 
 
-def run_nodes(raster, zoom, size, step, y, xa, xb):
+def last_node(t, size, lg, corner=False):
+    """the last lattice node tile t (along one axis) reads: its last pixel's centre, or its far corner, lies in the cell before it"""
+    return (((t + 1) * size - (0 if corner else 1)) >> lg) + 1
+
+
+def run_nodes(raster, zoom, size, step, y, xa, xb, corner=False):
     """(kx0, ky0, nodes) of the lattice that tiles xa..xb of tile row y read"""
     lg = step.bit_length() - 1
-    kx0, kx1 = (xa * size) >> lg, (((xb + 1) * size - 1) >> lg) + 1
-    ky0, ky1 = (y * size) >> lg, (((y + 1) * size - 1) >> lg) + 1
-    return kx0, ky0, lattice(raster, zoom, size, step, kx0, kx1, ky0, ky1)
+    kx0, kx1 = (xa * size) >> lg, last_node(xb, size, lg, corner)
+    ky0, ky1 = (y * size) >> lg, last_node(y, size, lg, corner)
+    return kx0, ky0, lattice(raster, zoom, size, step, kx0, kx1, ky0, ky1, corner)
 
 
 # ---- planning ----
@@ -252,27 +263,40 @@ def _lerp(a, b, t):
     return a + t * (b - a)
 
 
-def step_error(raster, zoom, size, step, run):
+def step_error(raster, zoom, size, step, run, corner=False):
     """the largest |exact - interpolated| (u or v, source pixels) at the lattice cell centres of a run; NaN cells are skipped"""
     y, xa, xb = run
-    kx0, ky0, nodes = run_nodes(raster, zoom, size, step, y, xa, xb)
+    kx0, ky0, nodes = run_nodes(raster, zoom, size, step, y, xa, xb, corner)
     mid = _lerp(_lerp(nodes[:-1, :-1], nodes[:-1, 1:], 0.5), _lerp(nodes[1:, :-1], nodes[1:, 1:], 0.5), 0.5)
     ny, nx = nodes.shape[0] - 1, nodes.shape[1] - 1
-    X = pixel_centre((np.arange(kx0, kx0 + nx, dtype=np.int64) * step).astype(np.float64) + step / 2, zoom, size)
-    Y = -pixel_centre((np.arange(ky0, ky0 + ny, dtype=np.int64) * step).astype(np.float64) + step / 2, zoom, size)
+    X = pixel_centre((np.arange(kx0, kx0 + nx, dtype=np.int64) * step).astype(np.float64) + step / 2, zoom, size, corner)
+    Y = -pixel_centre((np.arange(ky0, ky0 + ny, dtype=np.int64) * step).astype(np.float64) + step / 2, zoom, size, corner)
     u, v = source_coords(raster, *np.meshgrid(X, Y))
     err = np.maximum(np.abs(u - mid[..., 0]), np.abs(v - mid[..., 1]))
     err = err[np.isfinite(err)]
     return float(err.max()) if len(err) else 0.0
 
 
-def choose_step(raster, zoom, size, tiles):
+def choose_step(raster, zoom, size, tiles, corner=False):
     """the largest lattice step of STEPS that meets TOLERANCE on every run of `tiles`"""
     rs = runs(tiles)
     for step in STEPS:
-        if all(step_error(raster, zoom, size, step, r) <= TOLERANCE for r in rs):
+        if all(step_error(raster, zoom, size, step, r, corner) <= TOLERANCE for r in rs):
             return step
     return 1
+
+
+def footprint_bound(nodes, step):
+    """an upper bound of the unclipped extent (u1 - u0 or v1 - v0, source pixels) of every pixel footprint inside a block of corner
+    nodes [h, w, 2]: u is bilinear in each cell, so across one pixel (1 / step of a cell) it changes by at most (the largest |du| along
+    the cell's x edges + the largest along its y edges) / step; FOOTPRINT_SLACK covers the rounding of the interpolation. 0 when no
+    cell is finite."""
+    dx = np.abs(nodes[:, 1:] - nodes[:, :-1])  # [h, w - 1, 2]
+    dy = np.abs(nodes[1:] - nodes[:-1])  # [h - 1, w, 2]
+    with np.errstate(invalid="ignore"):
+        ext = (np.maximum(dx[:-1], dx[1:]) + np.maximum(dy[:, :-1], dy[:, 1:])) / step  # per cell and coordinate
+    ext = ext[np.isfinite(ext)]
+    return float(ext.max()) * (1 + 1e-12) + FOOTPRINT_SLACK if len(ext) else 0.0
 
 
 def source_box(nodes, raster):
@@ -307,21 +331,28 @@ def window_bytes(src_bytes, n, size, node_bytes):
     return src_bytes + n * size * size * 3 + node_bytes + n * 32 + 8
 
 
-def plan(raster, zoom, size, tiles, step, budget=DEFAULT_BUDGET, batch=DEFAULT_BATCH):
-    """the windows of `tiles` (int64 [n, 2], distinct); tiles whose lattice samples no raster pixel are in no window. RsbError
-    when one tile alone needs more than `budget` device bytes."""
+def plan(raster, zoom, size, tiles, step, budget=DEFAULT_BUDGET, batch=DEFAULT_BATCH, corner=False):
+    """the windows of `tiles` (int64 [n, 2], distinct) on the centre lattice, or the corner lattice of area averaging when `corner`;
+    tiles whose lattice samples no raster pixel are in no window. RsbError when one tile alone needs more than `budget` device
+    bytes, and, on the corner lattice, when a footprint of a tile may span more than RSB_TILE_MAX_FOOTPRINT source pixels."""
     lg = step.bit_length() - 1
     windows = []
     for y, xa, xb in runs(tiles):
-        kx0, ky0, nodes = run_nodes(raster, zoom, size, step, y, xa, xb)
+        kx0, ky0, nodes = run_nodes(raster, zoom, size, step, y, xa, xb, corner)
         cur = None
         for x in range(xa, xb + 1):
             a = ((x * size) >> lg) - kx0
-            b = ((((x + 1) * size - 1) >> lg) + 1) - kx0
+            b = last_node(x, size, lg, corner) - kx0
             box = source_box(nodes[:, a:b + 1], raster)
             if box is None:
                 cur = None
                 continue
+            if corner:
+                extent = footprint_bound(nodes[:, a:b + 1], step)
+                if extent > _lib.RSB_TILE_MAX_FOOTPRINT:
+                    raise _lib.RsbError("a pixel of tile (%d, %d, %d) may span %.1f source pixels, more than the %d that area averaging sums; "
+                                        "use a higher zoom (smaller tile pixels span fewer source pixels)" % (
+                                            x, y, zoom, extent, _lib.RSB_TILE_MAX_FOOTPRINT))
             alone = window_bytes(box[1] * box[3] * raster.spp, 1, size, nodes[:, a:b + 1].size * 8)
             if alone > budget:
                 raise _lib.RsbError("tile (%d, %d, %d) needs %d device bytes (a %d x %d source window), more than the budget of %d bytes" % (
@@ -350,6 +381,21 @@ def coarse_ratio(raster, zoom, size):
 
 # ---- execution ----
 
+def entry_point(resampling):
+    return "rsb_tile_average" if resampling == "average" else "rsb_tile_warp"
+
+
+def warp(lib, resampling, src, w, raster, nodes, step, tiles, n, size, out, image_stride, covered, misses):
+    """one launch of rsb_tile_warp or rsb_tile_average (device pointers) over Window `w`'s source and lattice, on the current stream"""
+    args = (src, w.cols * raster.spp, w.row0, w.col0, w.rows, w.cols, raster.width, raster.height, raster.spp, int(raster.alpha), raster.nodata,
+            nodes, w.kx0, w.ky0, w.nodes.shape[1], w.nodes.shape[0], step, tiles, n, size)
+    tail = (out, image_stride, covered, misses, _lib.current_stream_ptr())
+    if resampling == "average":
+        _lib.check(lib.rsb_tile_average(*args, *tail), "rsb_tile_average")
+    else:
+        _lib.check(lib.rsb_tile_warp(*args, RESAMPLING[resampling], *tail), "rsb_tile_warp")
+
+
 def _pinned(n):
     import torch
 
@@ -364,8 +410,8 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
     receives the lattice step and seconds of decode, upload, warp (CUDA events) and sink."""
     import torch
 
-    if resampling not in RESAMPLING:
-        raise ValueError("resampling must be one of %s" % ", ".join(RESAMPLING))
+    if resampling not in RESAMPLINGS:
+        raise ValueError("resampling must be one of %s" % ", ".join(RESAMPLINGS))
     if not 0 <= zoom <= _lib.RSB_COVER_MAX_ZOOM or not 1 <= size <= _lib.RSB_TILE_MAX_SIZE:
         raise ValueError("zoom must be in 0..%d and size in 1..%d" % (_lib.RSB_COVER_MAX_ZOOM, _lib.RSB_TILE_MAX_SIZE))
     stats = stats if stats is not None else {}
@@ -373,8 +419,9 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
     if tiles is not None:
         want = {(int(x), int(y)) for x, y in tiles}
         cand = cand[np.array([(int(x), int(y)) in want for x, y in cand], bool)] if len(cand) else cand
-    step = choose_step(raster, zoom, size, cand)
-    windows = plan(raster, zoom, size, cand, step, budget, batch)
+    corner = resampling == "average"
+    step = choose_step(raster, zoom, size, cand, corner)
+    windows = plan(raster, zoom, size, cand, step, budget, batch, corner)
     stats.update(step=step, candidates=len(cand), windows=len(windows), decode_s=0.0, upload_s=0.0, warp_s=0.0, sink_s=0.0, written=0)
     if not windows:
         return cand
@@ -387,7 +434,6 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
     out_host = [_pinned(nmax * size * size * 3) for _ in range(2)]
     counts_host = [torch.empty((nmax,), dtype=torch.int64, pin_memory=True) for _ in range(2)]
     misses_host = torch.empty((1,), dtype=torch.int64, pin_memory=True)
-    mode = RESAMPLING[resampling]
     lib = _lib.load()
 
     def decode(k):
@@ -432,10 +478,8 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
                 covered = torch.empty((n,), dtype=torch.int64, device=dev)
                 misses = torch.empty((1,), dtype=torch.int64, device=dev)
                 start.record(stream)
-                _lib.check(lib.rsb_tile_warp(src.data_ptr(), w.cols * spp, w.row0, w.col0, w.rows, w.cols, raster.width, raster.height, spp,
-                                             int(raster.alpha), raster.nodata, nodes.data_ptr(), w.kx0, w.ky0, w.nodes.shape[1], w.nodes.shape[0],
-                                             step, xy.data_ptr(), n, size, mode, out.data_ptr(), size * size * 3, covered.data_ptr(),
-                                             misses.data_ptr(), _lib.current_stream_ptr()), "rsb_tile_warp")
+                warp(lib, resampling, src.data_ptr(), w, raster, nodes.data_ptr(), step, xy.data_ptr(), n, size, out.data_ptr(), size * size * 3,
+                     covered.data_ptr(), misses.data_ptr())
                 end.record(stream)
                 if writes[k % 2] is not None:  # the writer is done with this buffer pair before it is overwritten
                     dt, kept = writes[k % 2].result()
@@ -447,8 +491,8 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
                 torch.cuda.synchronize(dev)
                 stats["warp_s"] += start.elapsed_time(end) / 1e3
                 if int(misses_host[0]):
-                    raise _lib.RsbError("rsb_tile_warp: %d samples of tiles %d..%d of row %d fell outside their source window (a planning error)" % (
-                        int(misses_host[0]), w.xs[0], w.xs[-1], w.y))
+                    raise _lib.RsbError("%s: %d samples of tiles %d..%d of row %d fell outside their source window (a planning error)" % (
+                        entry_point(resampling), int(misses_host[0]), w.xs[0], w.xs[-1], w.y))
                 del src, out
                 writes[k % 2] = writer.submit(deliver, k, n)
         finally:

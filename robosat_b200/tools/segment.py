@@ -16,7 +16,7 @@ def add_parser(subparser):
     parser.add_argument("--overlap", type=int, default=32, help="tile pixel overlap to predict on")
     parser.add_argument("--batch_size", type=int, default=32, help="tiles per batch")
     parser.add_argument("--tiles", type=str, default=None, help="only the tiles of this `rs cover` csv file")
-    parser.add_argument("--resampling", choices=["nearest", "bilinear"], default="bilinear", help="resampling of the image tiles")
+    parser.add_argument("--resampling", choices=["nearest", "bilinear", "average"], default="bilinear", help="resampling of the image tiles")
     parser.add_argument("--output", choices=["masks", "probs"], default="masks",
                         help="masks: class indices (as rs masks writes them); probs: foreground probability bins (two classes only)")
     parser.add_argument("--tta", type=str, default="none", choices=["none", "flip", "d4"],
@@ -85,13 +85,13 @@ def main(args, stats=None, budget=None):
     except (_lib.RsbError, OSError) as e:
         sys.exit("Error: %s" % e)
     ratio = T.coarse_ratio(raster, args.zoom, args.size)
-    if ratio > 2:
+    if ratio > 2 and args.resampling != "average":
         print(T.W_COARSE.format(args.zoom, ratio), file=sys.stderr)
     ratio = M.coarse_ratio(grid, args.zoom, args.size)
     if ratio > 2:
         print(M.W_COARSE.format(ratio, args.zoom), file=sys.stderr)
     try:
-        plan = SEG.plan(raster, grid, args.zoom, args.size, args.batch_size, listed, budget or SEG.DEFAULT_BUDGET)
+        plan = SEG.plan(raster, grid, args.zoom, args.size, args.batch_size, listed, budget or SEG.DEFAULT_BUDGET, args.resampling)
     except _lib.RsbError as e:
         sys.exit("Error: %s" % e)
     if not len(plan.tiles):

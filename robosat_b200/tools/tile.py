@@ -13,7 +13,7 @@ def add_parser(subparser):
     parser.add_argument("--zoom", type=int, required=True, help="zoom level of tiles")
     parser.add_argument("--size", type=int, default=512, help="size of image tiles in pixels")
     parser.add_argument("--tiles", type=str, default=None, help="only the tiles of this `rs cover` csv file")
-    parser.add_argument("--resampling", choices=["nearest", "bilinear"], default="bilinear", help="resampling method")
+    parser.add_argument("--resampling", choices=["nearest", "bilinear", "average"], default="bilinear", help="resampling method")
     parser.add_argument("raster", type=str, help="path to the GeoTIFF")
     parser.add_argument("out", type=str, help="directory to write the tiles to")
     parser.set_defaults(func=main)
@@ -58,7 +58,7 @@ def main(args, stats=None):
     except (_lib.RsbError, OSError) as e:
         sys.exit("Error: %s" % e)
     ratio = T.coarse_ratio(raster, args.zoom, args.size)
-    if ratio > 2:
+    if ratio > 2 and args.resampling != "average":
         print(T.W_COARSE.format(args.zoom, ratio), file=sys.stderr)
     threads = usable_cores()
 
