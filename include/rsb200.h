@@ -633,6 +633,41 @@ int rsb_tiff_decode_window(const uint8_t* file_host, int64_t file_len, const int
                            int32_t compression, int32_t predictor, int64_t row0, int64_t rows, int64_t col0, int64_t cols, uint8_t* out_host,
                            int32_t threads, int64_t* bad_chunk_host);
 
+/* JPEG (Compression 7) strips or tiles (DESIGN.md §8). Parse JPEGTables (tables_host [tables_len], tables_len 0 when absent) and
+ * the headers of the chunks select_host [num_select] (NULL: all num_chunks chunks, in order) of file_host (chunk_offsets_host,
+ * chunk_bytes_host, the raster and chunk sizes as rsb_tiff_decode_window; rows_per_strip is the TIFF's RowsPerStrip, at least
+ * chunk_h, and bounds a strip's frame height) on `threads` of the library's threads. spp 1 with photometric 1, or spp 3 with
+ * photometric 2 (RGB) or 6 (YCbCr). descs_host int64 [chunks parsed][RSB_JPEG_DESC_FIELDS], in parse order: the file offset and
+ * length of the chunk's entropy-coded bytes, its table set, frame width and height, luma sampling h and v, restart interval,
+ * block count, 0 (the first block, for the decoder), its index and 0. sets_host NULL: no table sets are built, the descriptors'
+ * table set is -1 and *num_sets_host = 0. Otherwise the distinct table sets of the parsed chunks, in order of first use, go to
+ * sets_host int32 [max_sets][RSB_JPEG_SET_WORDS] (quantisation tables in natural order, then per component libjpeg's derived DC and
+ * AC Huffman tables); *num_sets_host gets their count, and when it exceeds max_sets nothing is written to sets_host (call again
+ * with room). A stream outside the rule gives RSB_E_INVALID with a message starting "Compression 7 (JPEG)" that names the value
+ * found and the strip or tile, *bad_chunk_host = its index (-1 otherwise; may be NULL). Host only: no device needed. */
+#define RSB_JPEG_DESC_FIELDS 12
+#define RSB_JPEG_SET_WORDS 3480
+#define RSB_JPEG_SCRATCH_PER_BLOCK 192
+int rsb_jpeg_parse_chunks(const uint8_t* file_host, int64_t file_len, const uint8_t* tables_host, int64_t tables_len, const int64_t* chunk_offsets_host,
+                          const int64_t* chunk_bytes_host, int64_t num_chunks, int64_t width, int64_t height, int32_t chunk_w, int32_t chunk_h,
+                          int64_t rows_per_strip, int32_t tiled, int32_t spp, int32_t photometric, const int64_t* select_host, int64_t num_select,
+                          int32_t threads, int64_t* descs_host, int32_t* sets_host, int32_t max_sets, int32_t* num_sets_host, int64_t* bad_chunk_host);
+/* scratch bytes of rsb_jpeg_decode_window for total_blocks blocks: RSB_JPEG_SCRATCH_PER_BLOCK * total_blocks (-1 if negative) */
+int64_t rsb_jpeg_scratch_bytes(int64_t total_blocks);
+/* Decode raster rows [row0, row0 + rows) x columns [col0, col0 + cols) of a JPEG TIFF into out uint8 [rows][cols][spp] on `stream`
+ * (device pointers). The chunks the window touches, row-major over their rectangle, are descs int64 [num_chunks][RSB_JPEG_DESC_FIELDS]
+ * as rsb_jpeg_parse_chunks gives them, but with offsets into staged [staged_len] (their entropy-coded bytes) and first blocks
+ * ascending, each chunk's blocks inside [0, total_blocks); sets int32 [num_sets][RSB_JPEG_SET_WORDS]. scratch: at least
+ * rsb_jpeg_scratch_bytes(total_blocks) bytes, 16-byte aligned. errors int64 [num_chunks]: 0, or a data error code | MCU << 8 (1
+ * invalid Huffman code, 2 AC index past 63, 3 unexpected marker or RST number, 4 extraneous bytes before a marker, 5 data ends
+ * before the last MCU, 6 a descriptor outside the staged bytes, the scratch or the table sets, or inconsistent with its block
+ * count); the IDCT and pixel stages skip a chunk whose error word is not 0, so its pixels are left 0. Pixels follow libjpeg-turbo's default decompression (islow IDCT, fancy upsampling, integer YCbCr -> RGB for
+ * photometric 6). Arguments are validated before the device check; allocates nothing and does not synchronise. */
+int rsb_jpeg_decode_window(const uint8_t* staged, int64_t staged_len, const int64_t* descs, int32_t num_chunks, const int32_t* sets,
+                           int32_t num_sets, int64_t width, int64_t height, int32_t chunk_w, int32_t chunk_h, int32_t tiled, int32_t spp,
+                           int32_t photometric, int64_t row0, int64_t rows, int64_t col0, int64_t cols, uint8_t* out, void* scratch,
+                           int64_t scratch_bytes, int64_t total_blocks, int64_t* errors, void* stream);
+
 /* Warp N tiles of size x size of zoom z from a source window. src uint8 [win_rows][src_pitch] holds raster rows
  * [win_row0, + win_rows) x columns [win_col0, + win_cols) of a raster_w x raster_h image, spp (1, 3 or 4) samples per pixel (spp = 4:
  * 4-byte aligned rows). A pixel is valid unless alpha = 1 and its 4th sample is 0, or its colour samples (1 or 3) all equal nodata

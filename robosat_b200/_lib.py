@@ -107,6 +107,9 @@ RSB_COMPARE_MAX_CLASSES = 256
 RSB_TILE_MAX_SIZE = 4096
 RSB_TILE_MAX_STEP = 64
 RSB_TILE_MAX_FOOTPRINT = 64
+RSB_JPEG_DESC_FIELDS = 12
+RSB_JPEG_SET_WORDS = 3480
+RSB_JPEG_SCRATCH_PER_BLOCK = 192
 
 
 class MorphOp(ctypes.Structure):
@@ -251,6 +254,11 @@ SIGNATURES = {
     "rsb_png_write_rgb8_batch": (ctypes.c_int, [_vp, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _i32]),
     "rsb_tiff_decode_window": (ctypes.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64,
                                               _vp, _i32, _vp]),
+    "rsb_jpeg_parse_chunks": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i64, _i32, _i32, _i32, _vp, _i64, _i32,
+                                             _vp, _vp, _i32, _vp, _vp]),
+    "rsb_jpeg_scratch_bytes": (_i64, [_i64]),
+    "rsb_jpeg_decode_window": (ctypes.c_int, [_vp, _i64, _vp, _i32, _vp, _i32, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64, _vp,
+                                              _vp, _i64, _i64, _vp, _vp]),
     "rsb_tile_warp": (ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _vp, _i32,
                                      _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
     "rsb_tile_average": (ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _vp,

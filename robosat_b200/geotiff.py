@@ -2,10 +2,11 @@
 
 `GeoTiff(path)` parses IFD 0 and the GeoKeys with `struct` and checks that the image is one `rs tile` reads (DESIGN.md §8):
 8-bit unsigned chunky samples in strips or tiles, no compression, LZW or DEFLATE, predictor 1 or 2, and 1 band (MinIsBlack), 3
-(RGB) or 4 (RGB plus an alpha ExtraSample); georeferenced by one tiepoint plus a pixel scale or by an affine model transformation,
-in EPSG:3857, EPSG:4326 or a WGS 84 UTM zone (EPSG:32601-32660, 32701-32760). Anything else raises `RsbError` naming the value
-found. Overviews and sub-IFDs are ignored. `read_window` decodes a window of rows and columns with the library's decoder
-(`rsb_tiff_decode_window`) over a memory map of the file.
+(RGB) or 4 (RGB plus an alpha ExtraSample); or JPEG (Compression 7) with 1 band (MinIsBlack) or 3 (RGB, or YCbCr converted to RGB),
+every chunk's stream checked against the rule when the file is opened (robosat_b200/jpeg.py); georeferenced by one tiepoint plus
+a pixel scale or by an affine model transformation, in EPSG:3857, EPSG:4326 or a WGS 84 UTM zone (EPSG:32601-32660, 32701-32760).
+Anything else raises `RsbError` naming the value found. Overviews and sub-IFDs are ignored. `read_window` decodes a window of rows
+and columns with the library's decoder (`rsb_tiff_decode_window`) over a memory map of the file, or for JPEG on the device.
 
 `read_grid(path)` reads only the size and the georeferencing, with the same rules and messages for those, so any pixel layout
 (16-bit, JPEG, palette ...) is accepted: `rs mosaic --like` takes the grid of an existing raster.
@@ -22,7 +23,8 @@ from robosat_b200 import _lib
 
 TYPE_SIZES = {1: 1, 2: 1, 3: 2, 4: 4, 5: 8, 6: 1, 7: 1, 8: 2, 9: 4, 10: 8, 11: 4, 12: 8, 16: 8, 17: 8, 18: 8}
 TYPE_FORMATS = {1: "B", 2: "B", 3: "H", 4: "I", 5: "II", 6: "b", 7: "B", 8: "h", 9: "i", 10: "ii", 11: "f", 12: "d", 16: "Q", 17: "q", 18: "Q"}
-COMPRESSIONS = {1: "none", 5: "LZW", 8: "deflate", 32946: "deflate"}
+COMPRESSIONS = {1: "none", 5: "LZW", 7: "JPEG", 8: "deflate", 32946: "deflate"}
+JPEG = 7
 COMPRESSION_NAMES = {2: "CCITT RLE", 3: "CCITT fax 3", 4: "CCITT fax 4", 6: "old-style JPEG", 7: "JPEG", 32773: "PackBits", 34712: "JPEG 2000",
                      34887: "LERC", 34925: "LZMA", 50000: "Zstandard", 50001: "WebP"}
 PHOTOMETRIC_NAMES = {0: "MinIsWhite", 1: "MinIsBlack", 2: "RGB", 3: "palette", 4: "transparency mask", 5: "CMYK", 6: "YCbCr", 8: "CIELab"}
@@ -196,15 +198,42 @@ class _Header:
 
 class GeoTiff(_Header):
     """IFD 0 of a GeoTIFF. Attributes: width, height, spp (1, 3 or 4), alpha (the 4th sample is alpha), nodata (-1, or the 0..255
-    value of GDAL_NODATA), compression, predictor, tiled, chunk_w, chunk_h, offsets / byte_counts (int64 chunk table), epsg, crs
+    value of GDAL_NODATA), compression, predictor, photometric, tiled, chunk_w, chunk_h, offsets / byte_counts (int64 chunk table), epsg, crs
     (see `crs_of_epsg`) and geotransform (c, a, b, f, d, e): X = c + a u + b v, Y = f + d u + e v for raster coordinates (u, v),
-    pixel (i, j) covering [i, i + 1) x [j, j + 1) (PixelIsPoint tiepoints are shifted by half a pixel, as GDAL does)."""
+    pixel (i, j) covering [i, i + 1) x [j, j + 1) (PixelIsPoint tiepoints are shifted by half a pixel, as GDAL does). JPEG rasters
+    also have jpeg_tables (bytes or None) and jpeg_descs (robosat_b200.jpeg.parse); rows_per_strip is RowsPerStrip for strips."""
 
     def _parse(self):
         self._parse_tags()
         self._size()
         self._image()
         self._georeference()
+        if self.compression == JPEG:
+            from robosat_b200 import jpeg
+            from robosat_b200.hostinfo import usable_cores
+
+            tables = self._tags.get(347)
+            self.jpeg_tables = bytes(bytearray(tables)) if tables else None
+            self.jpeg_descs = jpeg.parse(self, self.file_bytes(), self.jpeg_tables, usable_cores())
+            self._decoder = None
+
+    def file_bytes(self):
+        """the file as a uint8 array over a read-only memory map"""
+        if self._map is None:
+            with open(self.path, "rb") as fp:
+                self._map = mmap.mmap(fp.fileno(), 0, access=mmap.ACCESS_READ)
+            self._buf = np.frombuffer(self._map, np.uint8)
+        return self._buf
+
+    def jpeg_decoder(self, device):
+        """the jpeg.Decoder of this raster on `device` (its table sets uploaded once)"""
+        import torch
+
+        from robosat_b200 import jpeg
+
+        if self._decoder is None or self._decoder.device != torch.device(device):
+            self._decoder = jpeg.Decoder(self, device)
+        return self._decoder
 
     def _image(self):
         t = self._tag
@@ -224,6 +253,13 @@ class GeoTiff(_Header):
             _fail(self.path, "SampleFormat %s is not supported; only 1 (unsigned integer) is" % (",".join(str(int(f)) for f in fmt)))
         photometric = int(t(262, (1 if self.spp == 1 else 2,))[0])
         extra = tuple(int(v) for v in t(338, ()))
+        if self.compression == JPEG and self.spp == 3 and photometric == 6:
+            photometric = 2  # YCbCr inside the JPEG streams, RGB out of the decoder
+            self.photometric = 6
+        else:
+            self.photometric = photometric
+        if self.compression == JPEG and self.spp not in (1, 3):
+            _fail(self.path, "Compression 7 (JPEG) with %d bands is not supported; use 1 (gray) or 3 (RGB or YCbCr)" % self.spp)
         if self.spp == 1 and photometric != 1:
             _fail(self.path, "one band with Photometric %d (%s) is not supported; only MinIsBlack is" % (photometric, PHOTOMETRIC_NAMES.get(photometric, "unknown")))
         if self.spp in (3, 4) and photometric != 2:
@@ -236,16 +272,18 @@ class GeoTiff(_Header):
         self.predictor = int(t(317, (1,))[0])
         if self.predictor not in (1, 2):
             _fail(self.path, "Predictor %d is not supported; use 1 or 2" % self.predictor)
-        if self.compression == 1:
-            self.predictor = 1  # libtiff applies the predictor only inside a codec; uncompressed data is stored as is
+        if self.compression in (1, JPEG):
+            self.predictor = 1  # libtiff applies the predictor only inside a codec other than JPEG; uncompressed data is stored as is
         if 322 in self._tags:
             self.tiled = True
             self.chunk_w, self.chunk_h = int(t(322)[0]), int(t(323, (0,))[0])
+            self.rows_per_strip = self.chunk_h
             offsets, counts = t(324), t(325)
             need = -(-self.width // max(1, self.chunk_w)) * -(-self.height // max(1, self.chunk_h))
         else:
             self.tiled = False
-            self.chunk_w, self.chunk_h = self.width, min(self.height, int(t(278, (2 ** 32 - 1,))[0]))
+            self.rows_per_strip = int(t(278, (2 ** 32 - 1,))[0])
+            self.chunk_w, self.chunk_h = self.width, min(self.height, self.rows_per_strip)
             offsets, counts = t(273), t(279)
             need = -(-self.height // max(1, self.chunk_h))
         if self.chunk_w < 1 or self.chunk_h < 1:
@@ -270,7 +308,8 @@ class GeoTiff(_Header):
     def read_window(self, row0, rows, col0, cols, out=None, threads=None):
         """raster rows [row0, row0 + rows) x columns [col0, col0 + cols) -> uint8 [rows, cols, spp] (into `out` when given, any
         C-contiguous uint8 array of at least that many bytes, e.g. pinned host memory); RsbError names a chunk that cannot be
-        decoded."""
+        decoded. A JPEG raster is decoded on the device (rsb_jpeg_decode_window) and copied back: it needs a GPU, and there is no
+        CPU decoder."""
         import ctypes
 
         from robosat_b200.hostinfo import usable_cores
@@ -279,10 +318,12 @@ class GeoTiff(_Header):
         if out is None:
             out = np.empty(n, np.uint8)
         view = np.frombuffer(out, np.uint8, n) if not isinstance(out, np.ndarray) else out.reshape(-1)[:n]
-        if self._map is None:
-            with open(self.path, "rb") as fp:
-                self._map = mmap.mmap(fp.fileno(), 0, access=mmap.ACCESS_READ)
-            self._buf = np.frombuffer(self._map, np.uint8)
+        if self.compression == JPEG:
+            from robosat_b200 import jpeg
+
+            jpeg.read_window(self, row0, rows, col0, cols, view)
+            return view.reshape(rows, cols, self.spp)
+        self.file_bytes()
         bad = ctypes.c_int64(-1)
         _lib.check(_lib.load().rsb_tiff_decode_window(self._buf.ctypes.data, self.file_len, self.offsets.ctypes.data, self.byte_counts.ctypes.data,
                                                        len(self.offsets), self.width, self.height, self.chunk_w, self.chunk_h, int(self.tiled),

@@ -54,7 +54,8 @@ class Plan:
     ops         [(kind, number, img_lo, img_hi, pl_lo, pl_hi)] in execution order, kind 'warp', 'predict' or 'mosaic'; the image
                 store holds indices [img_lo, img_hi) and the plane store [pl_lo, pl_hi) while the op runs
     wait        {k: batch}: warp k overwrites slots whose last reader was that batch's stitch (absent: no earlier reader)
-    image_slots, plane_slots, store_bytes: the peaks and what the two stores take
+    image_slots, plane_slots, store_bytes: the peaks and what the two stores take (for a JPEG raster, store_bytes also holds
+                decode_bytes: the staged bytes and decoder scratch of the largest warp window)
     """
 
 
@@ -98,6 +99,15 @@ def plan(raster, grid, zoom, size, batch=DEFAULT_BATCH, tiles=None, budget=DEFAU
         p.reach.append(np.array([[at.get((x, y), -1) for x in range(tx0, tx1 + 1)] for y in range(ty0, ty1 + 1)], np.int64))
     _schedule(p)
     p.store_bytes = p.image_slots * size * size * 3 + p.plane_slots * size * size
+    if T.is_jpeg(raster):  # the staged bytes and decoder scratch of the largest warp window count too
+        from robosat_b200 import jpeg
+
+        p.decode_bytes = max([jpeg.extra_bytes(raster, w.row0, w.rows, w.col0, w.cols) for w in p.warps], default=0)
+        p.store_bytes += p.decode_bytes
+        if p.store_bytes > budget:
+            raise _lib.RsbError("the image and plane stores and the JPEG decode need %d device bytes at their peak (%d tiles of %d x %d x 3, %d of "
+                                "%d x %d and %d bytes of staged chunks and decoder scratch), more than the budget of %d bytes; segment fewer tiles at "
+                                "once with --tiles" % (p.store_bytes, p.image_slots, size, size, p.plane_slots, size, size, p.decode_bytes, budget))
     if p.store_bytes > budget:
         raise _lib.RsbError("the image and plane stores need %d device bytes at their peak (%d tiles of %d x %d x 3 and %d of %d x %d), more than "
                             "the budget of %d bytes; segment fewer tiles at once with --tiles" % (
@@ -176,7 +186,8 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
     the class of each pixel (the soft vote of one model); 'probs' (two classes only): the foreground bins. sink(window, pixels) is
     called on a writer thread for every output window, in schedule order, with pixels uint8 [rows, cols] (None: every pixel is
     nodata). Returns the number of existing tiles. `stats`, a dict, receives the counts and the seconds of decode, warp, predict
-    (stitch, network, head and vote) and mosaic warp, the last three from CUDA events."""
+    (stitch, network, head and vote) and mosaic warp, the last three from CUDA events. For a JPEG raster, decode is the staging of the
+    chunks' entropy-coded bytes on the host; their upload and device decode run on the warps' stream, outside the warp events."""
     import torch
 
     from robosat_b200.hostinfo import usable_cores
@@ -209,10 +220,14 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
     main = torch.cuda.current_stream(dev)
     side = torch.cuda.Stream(device=dev)  # warps: their covered counts come back without waiting for the batches in flight
     spp = raster.spp
+    jpeg_host = T._jpeg_buffers(raster, p.warps, dev) if p.warps else None
     if p.warps:
         src_bytes = max(w.rows * w.cols * spp for w in p.warps)
         nmax = max(len(w.xs) for w in p.warps)
-        src_host = [torch.empty((src_bytes,), dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+        if jpeg_host:
+            src_host = jpeg_host["data"]
+        else:
+            src_host = [torch.empty((src_bytes,), dtype=torch.uint8, pin_memory=True) for _ in range(2)]
         src = torch.empty((src_bytes,), dtype=torch.uint8, device=dev)
         covered = torch.empty((nmax,), dtype=torch.int64, device=dev)
         misses = torch.zeros((2,), dtype=torch.int64, device=dev)
@@ -228,7 +243,10 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
     def decode(k):
         t0 = time.perf_counter()
         w = p.warps[k]
-        raster.read_window(w.row0, w.rows, w.col0, w.cols, out=src_host[k % 2].numpy(), threads=threads)
+        if jpeg_host:
+            jpeg_host["staged"][k % 2] = T._jpeg_stage(raster, w, jpeg_host, k % 2)
+        else:
+            raster.read_window(w.row0, w.rows, w.col0, w.cols, out=src_host[k % 2].numpy(), threads=threads)
         return time.perf_counter() - t0
 
     def deliver(m, pixels, done, counts):
@@ -251,7 +269,10 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
         nxt = decoder.submit(decode, k + 1) if k + 1 < len(p.warps) else None  # into the other pinned buffer, while this one warps
         with torch.cuda.stream(side):
             nbytes = w.rows * w.cols * spp
-            src[:nbytes].copy_(src_host[k % 2][:nbytes], non_blocking=True)
+            if jpeg_host:
+                keep = T._jpeg_decode(jpeg_host, k % 2, src[:nbytes])
+            else:
+                src[:nbytes].copy_(src_host[k % 2][:nbytes], non_blocking=True)
             nodes = torch.from_numpy(np.ascontiguousarray(w.nodes)).pin_memory().to(dev, non_blocking=True)
             xy = torch.from_numpy(p.tiles[a:b].copy()).pin_memory().to(dev, non_blocking=True)
             if k in p.wait:  # the stitch of that batch, or of the last batch before it that ran (stream order covers the rest)
@@ -271,6 +292,9 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
             counts_host[:b - a].copy_(covered[:b - a], non_blocking=True)
             counts_host[nmax:nmax + 2].copy_(misses, non_blocking=True)
         side.synchronize()  # the decode of window k + 2 reuses this window's pinned buffer; the counts decide what exists
+        if jpeg_host:
+            del keep
+            T._jpeg_check(jpeg_host, k % 2)
         missed = int(counts_host[nmax]) + int(counts_host[nmax + 1])
         if missed:
             raise _lib.RsbError("%s: %d samples of tiles %d..%d of row %d fell outside their source window (a planning error)" % (

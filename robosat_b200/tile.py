@@ -324,11 +324,26 @@ class Window:
         self.row0, self.rows, self.col0, self.cols = box
 
     def device_bytes(self, raster, size):
-        return window_bytes(self.rows * self.cols * raster.spp, len(self.xs), size, self.nodes.size * 8)
+        return window_bytes(source_bytes(raster, (self.row0, self.rows, self.col0, self.cols)), len(self.xs), size, self.nodes.size * 8)
 
 
 def window_bytes(src_bytes, n, size, node_bytes):
     return src_bytes + n * size * size * 3 + node_bytes + n * 32 + 8
+
+
+def is_jpeg(raster):
+    return getattr(raster, "compression", None) == 7
+
+
+def source_bytes(raster, box):
+    """device bytes of a source window (row0, rows, col0, cols): its pixels, plus for a JPEG raster the staged bytes and the decoder
+    scratch of the chunks it touches (jpeg.extra_bytes)"""
+    n = box[1] * box[3] * raster.spp
+    if is_jpeg(raster):
+        from robosat_b200 import jpeg
+
+        n += jpeg.extra_bytes(raster, *box)
+    return n
 
 
 def plan(raster, zoom, size, tiles, step, budget=DEFAULT_BUDGET, batch=DEFAULT_BATCH, corner=False):
@@ -353,7 +368,7 @@ def plan(raster, zoom, size, tiles, step, budget=DEFAULT_BUDGET, batch=DEFAULT_B
                     raise _lib.RsbError("a pixel of tile (%d, %d, %d) may span %.1f source pixels, more than the %d that area averaging sums; "
                                         "use a higher zoom (smaller tile pixels span fewer source pixels)" % (
                                             x, y, zoom, extent, _lib.RSB_TILE_MAX_FOOTPRINT))
-            alone = window_bytes(box[1] * box[3] * raster.spp, 1, size, nodes[:, a:b + 1].size * 8)
+            alone = window_bytes(source_bytes(raster, box), 1, size, nodes[:, a:b + 1].size * 8)
             if alone > budget:
                 raise _lib.RsbError("tile (%d, %d, %d) needs %d device bytes (a %d x %d source window), more than the budget of %d bytes" % (
                     x, y, zoom, alone, box[3], box[1], budget))
@@ -407,7 +422,8 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
     """Warp the candidate tiles of `raster` (a GeoTiff), intersected with `tiles` (iterable of (x, y)) when given. For every window,
     sink(xy int64 [n, 2], images uint8 [n, size, size, 3], covered int64 [n]) is called on a writer thread with the tiles that have
     covered pixels (the arrays are reused after the call returns). Returns the int64 [n, 2] candidate tiles. `stats`, a dict,
-    receives the lattice step and seconds of decode, upload, warp (CUDA events) and sink."""
+    receives the lattice step and seconds of decode, upload, warp (CUDA events) and sink. For a JPEG raster, decode is the staging of
+    the chunks' entropy-coded bytes on the host and upload includes their decode on the device."""
     import torch
 
     if resampling not in RESAMPLINGS:
@@ -429,7 +445,11 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
 
     dev = torch.device(device)
     spp = raster.spp
-    src_host = [_pinned(max(w.rows * w.cols * spp for w in windows)) for _ in range(2)]
+    jpeg_host = _jpeg_buffers(raster, windows, dev)
+    if jpeg_host:
+        src_host = jpeg_host["data"]
+    else:
+        src_host = [_pinned(max(w.rows * w.cols * spp for w in windows)) for _ in range(2)]
     nmax = max(len(w.xs) for w in windows)
     out_host = [_pinned(nmax * size * size * 3) for _ in range(2)]
     counts_host = [torch.empty((nmax,), dtype=torch.int64, pin_memory=True) for _ in range(2)]
@@ -439,7 +459,10 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
     def decode(k):
         t0 = time.perf_counter()
         w = windows[k]
-        raster.read_window(w.row0, w.rows, w.col0, w.cols, out=src_host[k % 2].numpy(), threads=threads)
+        if jpeg_host:
+            jpeg_host["staged"][k % 2] = _jpeg_stage(raster, w, jpeg_host, k % 2)
+        else:
+            raster.read_window(w.row0, w.rows, w.col0, w.cols, out=src_host[k % 2].numpy(), threads=threads)
         return time.perf_counter() - t0
 
     def deliver(k, n):
@@ -469,10 +492,16 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
                 n = len(w.xs)
                 t0 = time.perf_counter()
                 src = _alloc((w.rows * w.cols * spp,), torch.uint8, dev, "the %d x %d source window" % (w.cols, w.rows))
-                src.copy_(src_host[k % 2][:src.numel()], non_blocking=True)
+                if jpeg_host:
+                    keep = _jpeg_decode(jpeg_host, k % 2, src)
+                else:
+                    src.copy_(src_host[k % 2][:src.numel()], non_blocking=True)
                 nodes = torch.from_numpy(np.ascontiguousarray(w.nodes)).to(dev)
                 xy = torch.tensor([[x, w.y] for x in w.xs], dtype=torch.int64).to(dev)
                 torch.cuda.synchronize(dev)
+                if jpeg_host:
+                    del keep
+                    _jpeg_check(jpeg_host, k % 2)
                 stats["upload_s"] += time.perf_counter() - t0
                 out = _alloc((n, size, size, 3), torch.uint8, dev, "%d output tiles" % n)
                 covered = torch.empty((n,), dtype=torch.int64, device=dev)
@@ -502,6 +531,36 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
                     stats["sink_s"] += dt
                     stats["written"] += kept
     return cand
+
+
+def _jpeg_buffers(raster, windows, dev):
+    """for a JPEG raster: the decoder and two sets of pinned staging buffers sized for the largest of `windows`; None otherwise"""
+    import torch
+
+    if not is_jpeg(raster):
+        return None
+    from robosat_b200 import jpeg
+
+    nbytes, chunks = jpeg.stage_sizes(raster, [(w.row0, w.rows, w.col0, w.cols) for w in windows])
+    return dict(decoder=raster.jpeg_decoder(dev), data=[_pinned(nbytes) for _ in range(2)],
+                descs=[torch.empty((chunks * jpeg.F,), dtype=torch.int64, pin_memory=True) for _ in range(2)],
+                sets=[torch.empty((chunks * _lib.RSB_JPEG_SET_WORDS,), dtype=torch.int32, pin_memory=True) for _ in range(2)],
+                errors=[torch.empty((chunks,), dtype=torch.int64, pin_memory=True) for _ in range(2)], staged=[None, None])
+
+
+def _jpeg_stage(raster, w, bufs, i):
+    from robosat_b200 import jpeg
+
+    return jpeg.stage(raster, w.row0, w.rows, w.col0, w.cols, bufs["data"][i].numpy(), bufs["descs"][i].numpy(), bufs["sets"][i].numpy())
+
+
+def _jpeg_decode(bufs, i, src):
+    """the upload and decode of staging buffer i into the device window `src`, on the current stream"""
+    return bufs["decoder"].decode(bufs["staged"][i], bufs["data"][i], bufs["descs"][i], bufs["sets"][i], src, bufs["errors"][i])
+
+
+def _jpeg_check(bufs, i):
+    bufs["decoder"].check(bufs["staged"][i], bufs["errors"][i])
 
 
 def tile_device(raster, zoom, size, resampling="bilinear", tiles=None, budget=DEFAULT_BUDGET, batch=DEFAULT_BATCH, stats=None):
