@@ -386,6 +386,19 @@ extern "C" int rsb_rowconv_plan_create(const rsb_rowconv_desc* d, rsb_rowconv_pl
     if (split && !(d->mode == 1 && d->cin == 32 && d->taps_h == 3 && d->src.plane > 0 && (d->src.plane * 2) % 16 == 0))
         return set_error(RSB_E_INVALID, "rowconv: the strict-precision line buffer exists for the 3x3 32 -> 32 head layer only (needs src.plane)");
     const int planes = split ? 2 : 1;
+    // shared memory: the resident weights and the epilogue staging are fixed, the ring of input rows takes the rest and needs
+    // taps_h + 1 rows (e.g. the fused upsample 128 -> 64 does not fit: its weights alone take 128 KB)
+    const int buf_w = kRowTile + d->taps_w + d->nsub - 2;
+    const int slot_bytes = ((buf_w * cblk * 2 + 1023) / 1024) * 1024;
+    const int wblock_bytes = planes * d->Cout * cblk * 2;
+    const int stage = d->mode == 0 ? 2 * 2 * 64 * (d->Cout >= 64 ? 64 : 32) * 2 : 0;
+    const int fixed = d->nsub * d->taps_h * d->taps_w * cblocks * wblock_bytes + stage + 512 + 1088 + 1024;
+    const int row_bytes = slot_bytes * cblocks * planes;
+    const int ctas = 1;  // the two consumer warpgroups of one CTA take the whole register file
+    int slots = (232448 / ctas - 1024 - fixed) / row_bytes;
+    if (slots > kRowMaxSlots) slots = kRowMaxSlots;
+    if (slots < d->taps_h + 1)
+        return set_error(RSB_E_INVALID, "rowconv: needs %d bytes of shared memory for a %d-row ring", fixed + (d->taps_h + 1) * row_bytes, d->taps_h + 1);
     int rc = rsb_device_ok();
     if (rc) return rc;
 
@@ -400,10 +413,9 @@ extern "C" int rsb_rowconv_plan_create(const rsb_rowconv_desc* d, rsb_rowconv_pl
     kp.nphase_a = d->nphase_a;
     kp.dh0 = d->dh0;
     kp.dw0 = d->dw0;
-    kp.buf_w = kRowTile + d->taps_w + d->nsub - 2;
-    const int pb = cblk * 2;
-    kp.slot_bytes = ((kp.buf_w * pb + 1023) / 1024) * 1024;
-    kp.wblock_bytes = planes * d->Cout * pb;
+    kp.buf_w = buf_w;
+    kp.slot_bytes = slot_bytes;
+    kp.wblock_bytes = wblock_bytes;
     kp.plane_bytes = kp.slot_bytes * cblocks;
     kp.acc_scale = d->acc_scale != 0.f ? d->acc_scale : 1.f;
     kp.Wt = d->Wt;
@@ -457,17 +469,6 @@ extern "C" int rsb_rowconv_plan_create(const rsb_rowconv_desc* d, rsb_rowconv_pl
     plan->block_n = d->Cout;
     plan->mode = d->mode;
     plan->split = split;
-    // shared memory: weights + epilogue staging are fixed; the ring takes the rest
-    const int stage = d->mode == 0 ? 2 * 2 * 64 * (d->Cout >= 64 ? 64 : 32) * 2 : 0;
-    const int fixed = d->nsub * d->taps_h * d->taps_w * cblocks * kp.wblock_bytes + stage + 512 + 1088 + 1024;
-    const int row_bytes = kp.slot_bytes * cblocks * planes;
-    const int ctas = 1;  // the two consumer warpgroups of one CTA take the whole register file
-    int slots = (232448 / ctas - 1024 - fixed) / row_bytes;
-    if (slots > kRowMaxSlots) slots = kRowMaxSlots;
-    if (slots < d->taps_h + 1) {
-        delete plan;
-        return set_error(RSB_E_INVALID, "rowconv: needs %d bytes of shared memory for a %d-row ring", fixed + (d->taps_h + 1) * row_bytes, d->taps_h + 1);
-    }
     kp.slots = slots;
     plan->smem = slots * row_bytes + fixed;
     const int sms = num_sms();
@@ -510,7 +511,7 @@ extern "C" int rsb_rowconv_run(const rsb_rowconv_plan* plan, void* stream_) {
         case 64320222: return launch_row<64, 32, 0, 2, 2, 2>(plan, st);  // dec4: fused upsample 128 -> 32
         case 64640212: return launch_row<64, 64, 0, 2, 1, 2>(plan, st);  // fused upsample 64 -> 64
         case 64320212: return launch_row<64, 32, 0, 2, 1, 2>(plan, st);
-        case 64640222: return launch_row<64, 64, 0, 2, 2, 2>(plan, st);
+        // no fused upsample 128 -> 64: its resident weights leave no room for the row ring (rsb_rowconv_plan_create)
     }
     return set_error(RSB_E_INVALID, "rowconv: no kernel instance for cblk %d, Cout %d, mode %d, taps %d, cblocks %d, nsub %d", plan->cblk,
                      plan->block_n, plan->mode, k.taps_h, k.cblocks, k.nsub);

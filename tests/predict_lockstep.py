@@ -117,6 +117,20 @@ def strict_acc_bound(dd, parts):
     return P23 * (m_main + 17) * A + n * U * A + ll
 
 
+def conv_tol(dd, strict, val, mag, parts):
+    """elementwise tolerance of one convolution's outputs (the forms of the module docstring) from the float64 replay's
+    value, magnitude and parts (emulate.run_desc / run_rowdesc `sink`); the chain lengths come from descriptor `dd`"""
+    row = hasattr(dd, "taps_h")
+    K = dd.taps_h * dd.taps_w * dd.cin if row else 64 * sum(dd.segs[j].cblocks for j in range(dd.nseg))
+    if strict:
+        e = strict_acc_bound(dd, parts)
+        if dd.mode == 0:
+            e = e + 2 * U * mag
+            return e + P22 * (np.abs(val) + e) + P25
+        return e + 34 * U * mag
+    return ulp16(val) + K * U * mag if dd.mode == 0 else K * U * parts["dot"] + 34 * U * mag
+
+
 def op_kind(dd, strict):
     """report tag of a convolution from the executor's descriptor"""
     if hasattr(dd, "taps_h"):
@@ -275,21 +289,12 @@ class PredictLockstep(lockstep.Harness):
     def _ref_conv(self, dd, op):
         td = op.desc
         row = hasattr(td, "taps_h")
-        K = td.taps_h * td.taps_w * td.cin if row else 64 * sum(td.segs[j].cblocks for j in range(td.nseg))
         tag = op_kind(dd, self.strict)
         writes = []
 
         def sink(ptr, shape, strides, val, mag, parts, plane):
             idx, off = self._locate(ptr)
-            if self.strict:
-                e = strict_acc_bound(dd, parts)
-                if td.mode == 0:
-                    e = e + 2 * U * mag
-                    tol = e + P22 * (np.abs(val) + e) + P25
-                else:
-                    tol = e + 34 * U * mag
-            else:
-                tol = ulp16(val) + K * U * mag if td.mode == 0 else K * U * parts["dot"] + 34 * U * mag
+            tol = conv_tol(dd, self.strict, val, mag, parts)
             writes.append(_Write("%s out (%s)" % (op.name, self._blabel(idx)), idx, off, shape, strides, val, tol, tag, plane))
 
         (emulate.run_rowdesc if row else emulate.run_desc)(td, sink=sink)
