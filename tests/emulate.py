@@ -6,9 +6,23 @@ host-side logic (weight packing, parity views, upsample phases, window views, ou
 verified without a GPU.
 """
 
+import concurrent.futures
 import ctypes
+import os
 
 import numpy as np
+
+WORKERS = max(1, min(16, len(os.sched_getaffinity(0))))
+
+
+def pmap(fn, items):
+    """[fn(x) for x in items] on a thread pool: the float64 references are numpy work on large arrays, which runs outside the
+    interpreter lock, so independent chunks use the host's cores"""
+    items = list(items)
+    if len(items) < 2:
+        return [fn(x) for x in items]
+    with concurrent.futures.ThreadPoolExecutor(min(len(items), WORKERS)) as ex:
+        return list(ex.map(fn, items))
 
 
 def _view(ptr, shape, strides_elems, dtype=np.float16, writable=False):
@@ -164,6 +178,80 @@ def _gather(sv, src, dh, dw, Nt, Ht, Wt, width):
     nn = min(Nt, src.N)
     a[:nn, :, :, :g.shape[-1]] = g[:nn]
     return a
+
+
+def _gather_at(sv, src, dh, dw, n, y, x, width):
+    """A operand rows of one tap at output pixels (n, y, x) (int64 arrays): [S, width] of the view `sv` [N, H, W, C] at
+    (n, y + dh, x + dw), zero outside the view (as _gather)"""
+    hh, ww = y + dh, x + dw
+    inb = (hh >= 0) & (hh < src.H) & (ww >= 0) & (ww < src.W) & (n < src.N)
+    c = min(width, sv.shape[-1])
+    g = sv[np.minimum(n, src.N - 1), np.clip(hh, 0, src.H - 1), np.clip(ww, 0, src.W - 1), :c] * inb[:, None]
+    if c == width:
+        return g
+    a = np.zeros((len(n), width), dtype=g.dtype)
+    a[:, :c] = g
+    return a
+
+
+def conv_out_views(d):
+    """(phase, byte address, shape, element strides) of every output phase of a mode-0 descriptor, as the kernel addresses them"""
+    strides = (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1)
+    return [(ph, d.out + 2 * ((ph >> 1) * d.out_pitch_h + (ph & 1) * d.out_pitch_w), (d.Nt, d.Ht, d.Wt, d.Cout), strides)
+            for ph in range(d.phases)]
+
+
+def conv_f64_at(d, pix):
+    """The float64 reference of mode-0 descriptor `d` (what run_desc(d, sink) gives) at sampled output pixels only.
+    pix: int64 [S, 3] (n, y, x) in the tile space, or [S, 4] with the output phase (2 pa + pb) of a 4-phase decoder last.
+    Returns (value, mag, addr): value and mag [S, Cout] as the sink receives them (mag = sum |a||w| (+ |bias| + |residual|),
+    with the (hi, lo) pair magnitudes in split mode) and addr [S], the byte address of channel 0 of each pixel's output (the
+    lo plane of a split output lies d.out_plane elements further)."""
+    assert d.mode == 0, "conv_f64_at: head descriptors are checked whole"
+    pix = np.asarray(pix, dtype=np.int64)
+    if pix.shape[1] == 3:
+        assert d.phases == 1
+        pix = np.concatenate([pix, np.zeros((len(pix), 1), np.int64)], axis=1)
+    split = bool(d.split)
+    K = 64 * sum(d.segs[i].cblocks for i in range(d.nseg))
+    rows = d.phases * d.Cout
+    w = _operand(d.weights, rows * K if split else 0, (rows, K), (K, 1))
+    # fp16 views of the sources (and their lo planes): only the gathered rows are converted to float64
+    srcs = [tuple(None if pl is None else _view(s.ptr + 2 * pl, (s.N, s.H, s.W, s.C), (s.pitch_n, s.pitch_h, s.pitch_w, 1))
+                  for pl in (0, s.plane if split else None))
+            for s in (d.srcs[i] for i in range(d.nsrc))]
+    scale = float(d.acc_scale) if d.acc_scale != 0 else 1.0
+    S = len(pix)
+    val, mag, addr = np.zeros((S, d.Cout)), np.zeros((S, d.Cout)), np.zeros(S, dtype=np.int64)
+    for phase, base, _, strides in conv_out_views(d):
+        sel = np.nonzero(pix[:, 3] == phase)[0]
+        if not sel.size:
+            continue
+        n, y, x = pix[sel, 0], pix[sel, 1], pix[sel, 2]
+        assert (n >= 0).all() and (n < d.Nt).all() and (y >= 0).all() and (y < d.Ht).all() and (x >= 0).all() and (x < d.Wt).all()
+        pa, pb = phase >> 1, phase & 1
+        acc = _F64Acc(split)
+        k0 = 0
+        for si in range(d.nseg):
+            seg = d.segs[si]
+            width = seg.cblocks * 64
+            a = tuple(None if p is None else _gather_at(p, d.srcs[seg.src], seg.dh + pa, seg.dw + pb, n, y, x, width).astype(np.float64)
+                      for p in srcs[seg.src])
+            acc.add(a, tuple(None if p is None else p[phase * d.Cout:(phase + 1) * d.Cout, k0:k0 + width] for p in w))
+            k0 += width
+        v, m = acc.val * scale, acc.dot * scale
+        if d.bias:
+            b = _view(d.bias, (d.Cout,), (1,), np.float32).astype(np.float64)
+            v, m = v + b, m + np.abs(b)
+        eoff = n * strides[0] + y * strides[1] + x * strides[2]
+        if d.residual:
+            rbase = d.residual + (base - d.out)
+            r = _pair(rbase, d.res_plane if split else 0, (d.Nt, d.Ht, d.Wt, d.Cout), strides)[n, y, x]
+            v, m = v + r, m + np.abs(r)
+        val[sel] = np.maximum(v, 0) if d.relu else v
+        mag[sel] = m
+        addr[sel] = base + 2 * eoff
+    return val, mag, addr
 
 
 def run_desc(d, sink=None):
@@ -354,6 +442,58 @@ def run_wgrad(d, dy_ptr, dw, f64=False):
             k0 += a.shape[-1]
     if f64:
         return out, mag
+
+
+def _band(sv, src, dh, dw, n, h0, h1, Wt, width):
+    """A operand of one tap for output rows h0:h1 of image n: [h1 - h0, Wt, width] float64 of the view `sv` [N, H, W, C] shifted
+    by (dh, dw), zero outside the view (as _gather)"""
+    a = np.zeros((h1 - h0, Wt, width))
+    ya, yb = max(h0, -dh), min(h1, src.H - dh)
+    xa, xb = max(0, -dw), min(Wt, src.W - dw)
+    if n < src.N and ya < yb and xa < xb:
+        c = min(width, sv.shape[-1])
+        a[ya - h0:yb - h0, xa:xb, :c] = sv[n, ya + dh:yb + dh, xa + dw:xb + dw, :c]
+    return a
+
+
+def run_wgrad_rows(d, dy_ptr, rows, chunk_bytes=64 << 20):
+    """rows `rows` (indices into the phases*Cout rows of the packed gradient) of run_wgrad(d, dy_ptr, None, f64=True), all K
+    columns, in float64 over all pixels. The A operand is gathered in bands of output rows of at most `chunk_bytes` of float64
+    per segment, the bands in parallel. Returns (gradient, magnitude), both [len(rows), K]."""
+    rows = np.asarray(rows, dtype=np.int64)
+    K = 64 * sum(d.segs[i].cblocks for i in range(d.nseg))
+    out, mag = np.zeros((len(rows), K)), np.zeros((len(rows), K))
+    band = max(1, min(d.Ht, chunk_bytes // (8 * K * d.Wt)))
+    svs = [_view(s.ptr, (s.N, s.H, s.W, s.C), (s.pitch_n, s.pitch_h, s.pitch_w, 1)) for s in (d.srcs[i] for i in range(d.nsrc))]
+    for phase in range(d.phases):
+        sel = np.nonzero(rows // d.Cout == phase)[0]
+        if not sel.size:
+            continue
+        co = rows[sel] % d.Cout
+        pa, pb = phase >> 1, phase & 1
+        base = dy_ptr + 2 * (pa * d.out_pitch_h + pb * d.out_pitch_w)
+        dyv = _view(base, (d.Nt, d.Ht, d.Wt, d.Cout), (d.out_pitch_n, d.out_sy * d.out_pitch_h, d.out_sx * d.out_pitch_w, 1))
+
+        def part(task):
+            n, h0 = task
+            h1 = min(d.Ht, h0 + band)
+            g = dyv[n, h0:h1][..., co].astype(np.float64).reshape(-1, len(co))  # [pixels, rows]
+            ga = np.abs(g)
+            o, m = np.zeros((len(co), K)), np.zeros((len(co), K))
+            k0 = 0
+            for si in range(d.nseg):
+                seg = d.segs[si]
+                width = seg.cblocks * 64
+                a = _band(svs[seg.src], d.srcs[seg.src], seg.dh + pa, seg.dw + pb, n, h0, h1, d.Wt, width).reshape(-1, width)
+                o[:, k0:k0 + width] = g.T @ a
+                m[:, k0:k0 + width] = ga.T @ np.abs(a)
+                k0 += width
+            return o, m
+
+        for o, m in pmap(part, [(n, h0) for n in range(d.Nt) for h0 in range(0, d.Ht, band)]):
+            out[sel] += o
+            mag[sel] += m
+    return out, mag
 
 
 def run_train_ops(eng, ops, x=None, dlogits=None):

@@ -26,21 +26,23 @@ that sit next to a rounding boundary. A is the float64 sum of the magnitudes of 
                            partial products of 16 terms each into an fp32 accumulator (bound as for wgrad below):
                            (K/16 + 17) * 2^-23 * A <= K * 2^-24 * A for K >= 64.
   conv stats  partials     sum of the partial rows vs float64 column sums / sums of squares of the kernel's own fp16 z:
-                           rel 1e-5 of sum |z| / sum z^2 (each partial adds 32 rows in fp32, 32 u = 1.9e-6).
+                           gamma_31 of sum |z| / sum z^2 (each partial adds 32 rows in fp32: 31 roundings).
   wgrad       fp32 dw      2^-23 * (P/16 + P/64 + 17) * A, A = sum_p |dy_p| |x_p|: P/16 accumulator additions of 16-pixel MMAs,
                            at most P/64 slice partials added afterwards (a slice holds at least one 64-pixel tile), and the
                            sum inside each MMA: its 16 products are aligned to the largest one and truncated, so each can lose
                            2^-23 of that block maximum, at most 16 * 2^-23 * A over all blocks (+1 for the normalisation).
                            Layers with fewer than 16 pixels per phase (center, dec0) need that term: measured errors there
                            reach 2-4 fp32 ulps of a result made of a handful of same-sign products.
-  bn_stats    mean etc.    from the sums' error e_s = 1e-5 relative to sum |z| (<= ~160 fp32 additions per partial before the
-                           fp64 accumulation: 160 u < 1e-5): d_mean = e_s E|z| + u |mean|, d_var = e_s E[z^2] + 2 |mean| d_mean,
+  bn_stats    mean etc.    from the sums' error e_s = e_sum(partial_reduce launch) relative to sum |z| (tests/train_launch.py derives
+                           it from the launch geometry: the 32-row conv-stats partials, the rows each thread folds, the shared-
+                           memory fold, then fp64): d_mean = e_s E|z| + u |mean|, d_var = e_s E[z^2] + 2 |mean| d_mean,
                            d_invstd = invstd (d_var / 2 (var + eps) + 2u), d_scale = |gamma| d_invstd + u |scale|,
                            d_shift = |mean| d_scale + |scale| d_mean + 2u (|beta| + |mean scale|); running stats: momentum
                            times those plus 4u of their magnitudes; num_batches_tracked exact.
   bn_apply    fp16 y       ulp16(ref) + 2^-23 (|z scale| + |shift| + |res|): one fma and one add in fp32, then fp16.
   bn_bwd      dz           ulp16(ref) + 2^-22 (|A g| + |B z| + |D|) + |A| (d_s0 + |zhat| d_s1) / M, with dz = A g + B z + D the
-                           kernel's fp32 form, d_s0 = e_s sum |g| and d_s1 = e_s invstd (sum |g z| + |mean| sum |g|)
+                           kernel's fp32 form, d_s0 = e_s sum |g| and d_s1 = e_s invstd (sum |g z| + |mean| sum |g|),
+                           e_s = e_sum(channel_reduce launch)
                            (the kernel forms sum g zhat as (sum g z - mean sum g) invstd);
               g_out        exact (a masked copy);
               dgamma/dbeta d_s1 / loss_scale + 2u |ref|, d_s0 / loss_scale + 2u |ref|.
@@ -49,8 +51,20 @@ that sit next to a rounding boundary. A is the float64 sum of the magnitudes of 
   pack_all    fp16 packed  exact for single-source layouts (one rounding of the fp32 weight); ulp16(ref) + 2^-22 A for the
                            pre-summed upsample taps (<= 3 fp32 additions, then fp16).
   final_fwd   fp32 logits  34 u A (32 fmas + the bias, A = sum |w y| + |b|).
-  final_bwd   fp16 dy5     ulp16(ref) + (C + 2) u A; dW, db: e_s A + 2u |ref| (fp32 per-thread partials, fp64 totals).
+  final_bwd   fp16 dy5     ulp16(ref) + (C + 2) u A; dW, db: e_s A + 2u |ref|, e_s = e_sum(final_bwd_dw launch) (fp32
+                           per-thread partials and a warp shuffle tree, fp64 totals).
   unpack_all  fp32 grads   2^-22 A + 2u |ref| (<= 4 fp32 additions and the 1/loss_scale product).
+
+Sampled mode (Lockstep(..., sample_above=n), for the shapes the benchmark trains at): a convolution (forward or .dgrad) with more
+than n output pixels is compared at sampled pixels only -- for every image the whole first, last (ragged) and one seeded random
+tile box of the kernel's own tiling (TW x TH x TN from the descriptor), the four corners and 256 seeded random pixels, all Cout
+channels, every phase -- with emulate.conv_f64_at; a weight gradient of such a layer at rows 0, 63, 64, 127, 128, the last and
+4 seeded random rows, all K columns, with emulate.run_wgrad_rows. The stray-write check and the teacher forcing still cover
+the op's whole output, and every other op is checked element by element in chunks of at most `chunk` elements, so the host
+memory of the references stays bounded. The chunks run on a thread pool (emulate.pmap).
+
+The stray-write snapshot lives on the executor's device, or, with snapshot="host", one host copy per buffer: each op then
+pulls every tracked buffer back to compare it, slower but without a second copy of the engine on the device.
 """
 
 import bisect
@@ -60,9 +74,10 @@ import torch
 import torch.nn.functional as F
 
 import emulate
+import train_launch
 
 U = 2.0 ** -24
-E_SUM = 1e-5
+E_CONV_STATS = train_launch.conv_stats_partial()  # the conv epilogue's 32-row fp32 partial sums
 BN_EPS = 1e-5
 BN_MOMENTUM = 0.1
 
@@ -75,8 +90,9 @@ class LockstepError(AssertionError):
 
 def ulp16(x):
     """spacing of fp16 numbers at |x| (the subnormal spacing 2^-24 below 2^-14)"""
-    e = np.floor(np.log2(np.maximum(np.abs(x), 2.0 ** -14)))
-    return np.exp2(e - 10)
+    m = np.maximum(np.abs(np.asarray(x, dtype=np.float64)), 2.0 ** -14)
+    p2 = (m.view(np.int64) & np.int64(0x7FF0000000000000)).view(np.float64)  # 2^floor(log2 m), exactly
+    return np.where(np.isnan(m), np.nan, p2 * 2.0 ** -10)
 
 
 def _f64(t):
@@ -126,13 +142,16 @@ class GpuExecutor:
 class _Write:
     """an output view (base buffer index, element offset, shape, element strides) with its reference and tolerance.
     plane > 0: the output is an fp16 (hi, lo) pair whose lo plane lies `plane` elements behind the hi plane; the value
-    compared with the reference is hi + lo."""
+    compared with the reference is hi + lo.
+    sample: the reference covers only these elements (absolute element offsets into the base buffer, ref's shape).
+    fn: the reference is computed lazily, fn(a, b) -> (ref, tol) for rows a:b of the view's first axis, chunk by chunk; fn reads
+    the twin before the chunk's outputs are copied into it (an op that writes in place reads only the chunk it writes)."""
 
-    __slots__ = ("label", "idx", "off", "shape", "strides", "ref", "tol", "tag", "plane")
+    __slots__ = ("label", "idx", "off", "shape", "strides", "ref", "tol", "tag", "plane", "sample", "fn")
 
-    def __init__(self, label, idx, off, shape, strides, ref, tol, tag, plane=0):
+    def __init__(self, label, idx, off, shape, strides, ref, tol, tag, plane=0, sample=None, fn=None):
         self.label, self.idx, self.off, self.shape, self.strides = label, idx, off, tuple(shape), tuple(strides)
-        self.ref, self.tol, self.tag, self.plane = ref, tol, tag, plane
+        self.ref, self.tol, self.tag, self.plane, self.sample, self.fn = ref, tol, tag, plane, sample, fn
 
     def offsets(self):
         return (self.off, self.off + self.plane) if self.plane else (self.off,)
@@ -158,6 +177,35 @@ def _same(a, b):
     x, y = a.reshape(-1).view(torch.uint8).numpy(), b.reshape(-1).view(torch.uint8).numpy()
     n = x.size - x.size % 8
     return np.array_equal(x[:n].view(np.int64), y[:n].view(np.int64)) and np.array_equal(x[n:], y[n:])
+
+
+def _judge(tag, got, ref, tol, where):
+    """elementwise check of one piece of an output. Returns (worst err/tol, or the worst |err| of an exact check; exact?;
+    elements out of tolerance; (err/tol, position, got, ref, tol) of the worst of them or None; bn_apply outputs one fp16 ulp
+    from the correctly rounded value; bn_apply elements)"""
+    tol = np.broadcast_to(np.asarray(tol, dtype=np.float64), ref.shape)
+    err = np.abs(got - ref)
+    nan = np.isnan(err)
+    if nan.any():  # NaN where both are NaN is a match, any other NaN an unbounded error
+        err = np.where(nan, np.where(np.isnan(got) & np.isnan(ref), 0.0, np.inf), err)
+    exact = not np.any(tol)
+    if exact:
+        ratio = float(err.max()) if err.size else 0.0
+        bad = err > 0
+    else:
+        q = np.divide(err, tol, out=np.where(err > 0, np.inf, 0.0), where=tol > 0)
+        ratio = float(q.max()) if q.size else 0.0
+        bad = err > tol
+    flips = elems = 0
+    if tag == "bn_apply":
+        elems = got.size
+        flips = int(np.count_nonzero(got != ref.astype(np.float16).astype(np.float64)))
+    nbad, worst = int(np.count_nonzero(bad)), None
+    if nbad:
+        score = np.where(bad, err / np.maximum(tol, 1e-300), -1)
+        k = int(np.argmax(score))
+        worst = (float(score.reshape(-1)[k]), where(k), float(got.reshape(-1)[k]), float(ref.reshape(-1)[k]), float(tol.reshape(-1)[k]))
+    return ratio, exact, nbad, worst, flips, elems
 
 
 class Harness:
@@ -219,6 +267,10 @@ class Harness:
             by_base.setdefault(w.idx, []).append(w)
         for b in self.tracked:
             cur, snap = self.db[b], self.snap[b]
+            if cur.device != snap.device:  # host snapshot: a buffer the op does not write is compared through a device staging
+                if b not in by_base and self._same_as_host(cur, snap):
+                    continue
+                cur = cur.cpu()
             if b not in by_base:
                 if _same(cur, snap):
                     continue
@@ -239,36 +291,69 @@ class Harness:
             snap.copy_(cur)
             self.tb[b].copy_(self._pull(b))  # the twin follows, so later ops are checked on what the executor really holds
 
+    def _same_as_host(self, cur, snap):
+        """bit equality of device buffer cur and its pinned host snapshot, uploaded in pieces through one staging buffer"""
+        c, h = cur.reshape(-1).view(torch.uint8), snap.reshape(-1).view(torch.uint8)
+        if self._stage is None or self._stage.device != cur.device:
+            self._stage = torch.empty(256 << 20, dtype=torch.uint8, device=cur.device)
+        n = self._stage.numel()
+        for a in range(0, c.numel(), n):
+            m = min(n, c.numel() - a)
+            self._stage[:m].copy_(h[a:a + m], non_blocking=True)
+            if not torch.equal(self._stage[:m], c[a:a + m]):
+                return False
+        return True
+
     def _compare(self, which, i, ot, w):
-        got_t = [self._dut_view(w.idx, off, w.shape, w.strides).cpu() for off in w.offsets()]
-        got = sum(t.double() for t in got_t).numpy()
-        ref = np.asarray(w.ref, dtype=np.float64)
-        tol = np.broadcast_to(np.asarray(w.tol, dtype=np.float64), ref.shape)
-        err = np.abs(got - ref)
-        err = np.where(np.isnan(err) & ~(np.isnan(got) & np.isnan(ref)), np.inf, err)
-        err = np.where(np.isnan(err), 0.0, err)
-        exact = not np.any(tol)
-        st = self.stats.setdefault(w.tag, [0, 0.0, exact])
+        st = self.stats.setdefault(w.tag, [0, 0.0, True])
         st[0] += 1
-        st[2] = st[2] and exact
-        if exact:
-            worst = float(err.max()) if err.size else 0.0
-            st[1] = max(st[1], worst)
-            bad = err > 0
+        if w.sample is not None:
+            flat = self.db[w.idx].reshape(-1)
+            got = sum(flat[torch.from_numpy(w.sample.reshape(-1) + (off - w.off)).to(flat.device)].double().cpu()
+                      for off in w.offsets()).numpy().reshape(w.sample.shape)
+            res = [_judge(w.tag, got, w.ref, w.tol, lambda k: np.unravel_index(int(w.sample.reshape(-1)[k]), tuple(self.tb[w.idx].shape)))]
+            for off in w.offsets():
+                _view(self.tb[w.idx], off, w.shape, w.strides).copy_(self._dut_view(w.idx, off, w.shape, w.strides).cpu())
+        elif w.fn is None:
+            got_t = [self._dut_view(w.idx, off, w.shape, w.strides).cpu() for off in w.offsets()]
+            got = sum(t.double() for t in got_t).numpy()
+            ref = np.asarray(w.ref, dtype=np.float64)
+            res = [_judge(w.tag, got, ref, w.tol, lambda k: np.unravel_index(k, ref.shape))]
+            for off, t in zip(w.offsets(), got_t):
+                _view(self.tb[w.idx], off, w.shape, w.strides).copy_(t)
         else:
-            ratio = np.divide(err, tol, out=np.where(err > 0, np.inf, 0.0), where=tol > 0)
-            st[1] = max(st[1], float(ratio.max()) if ratio.size else 0.0)
-            bad = err > tol
-        if w.tag == "bn_apply":
-            self.bn_apply_elems += got.size
-            self.ulp_flips += int((got != ref.astype(np.float16).astype(np.float64)).sum())
-        if bad.any():
-            k = int(np.argmax(np.where(bad, err / np.maximum(tol, 1e-300), -1)))
-            pos = np.unravel_index(k, ref.shape)
+            lead, inner = w.shape[0], int(np.prod(w.shape[1:]))
+            step = max(1, self.chunk // max(inner, 1))
+
+            def piece(a):
+                # one chunk: its reference (read from the twin before the chunk's outputs are copied into it), the check, the copy
+                b = min(lead, a + step)
+                shape = (b - a,) + w.shape[1:]
+                offs = [off + a * w.strides[0] for off in w.offsets()]
+                got_t = [self._dut_view(w.idx, off, shape, w.strides).cpu() for off in offs]
+                got = sum(t.double() for t in got_t).numpy()
+                ref, tol = w.fn(a, b)
+                r = _judge(w.tag, got, np.asarray(ref, dtype=np.float64).reshape(shape), tol,
+                           lambda k: (lambda p: (p[0] + a,) + p[1:])(np.unravel_index(k, shape)))
+                for off, t in zip(offs, got_t):
+                    _view(self.tb[w.idx], off, shape, w.strides).copy_(t)
+                return r
+
+            res = emulate.pmap(piece, range(0, lead, step))
+        nbad, worst = 0, None
+        for ratio, exact, bad, wst, flips, elems in res:
+            st[1] = max(st[1], ratio)
+            st[2] = st[2] and exact
+            if elems:
+                self.ulp_flips += flips
+                self.bn_apply_elems += elems
+            nbad += bad
+            if wst is not None and (worst is None or wst[0] > worst[0]):
+                worst = wst
+        if nbad:
+            _, pos, g, r, t = worst
             self._fail(which, i, ot, w.label, "%d element(s) out of tolerance; worst at %s: got %r, float64 reference %r, tolerance %r" % (
-                int(bad.sum()), tuple(int(v) for v in pos), float(got.reshape(-1)[k]), float(ref.reshape(-1)[k]), float(tol.reshape(-1)[k])))
-        for off, t in zip(w.offsets(), got_t):
-            _view(self.tb[w.idx], off, w.shape, w.strides).copy_(t)
+                nbad, tuple(int(v) for v in pos), g, r, t))
 
     def table(self):
         lines = ["%-22s %7s  %s" % ("kind", "checks", "worst err/tol (exact kinds: worst |err|)")]
@@ -281,8 +366,14 @@ class Harness:
 class Lockstep(Harness):
     """the training plan: fwd_ops then bwd_ops of a UNetTrainEngine"""
 
-    def __init__(self, dut, twin):
+    def __init__(self, dut, twin, sample_above=None, chunk=1 << 22, sms=train_launch.SMS, seed=0, snapshot="device"):
+        """sample_above: sampled mode for convolutions with more output pixels and their weight gradients (see above);
+        chunk: elements per piece of the chunked elementwise checks; sms: the device's SM count (the bn_stats grid reads it);
+        snapshot: "device" or "host", where the stray-write check keeps its copy of the executor's buffers"""
         self.dut, self.tw = dut, twin
+        self.sample_above, self.chunk, self.seed = sample_above, chunk, seed
+        self.launches = train_launch.plan_launches(twin, sms=sms)
+        self.launch = train_launch.by_op(self.launches)
         E, T = dut.eng, twin
         assert T.plan_only and T.device.type == "cpu"
         self.db, self.tb = _bases(E), _bases(T)
@@ -324,7 +415,11 @@ class Lockstep(Harness):
         # the executor's state is the starting point: copy it into the twin once, snapshot it on the executor's device
         for i in self.tracked:
             self.tb[i].copy_(self.db[i].cpu())
-        self.snap = {i: self.db[i].clone() for i in self.tracked}
+        if snapshot == "host" and self.db[0].device.type != "cpu":
+            self.snap = {i: self.db[i].cpu().pin_memory() for i in self.tracked}
+        else:
+            self.snap = {i: self.db[i].clone() for i in self.tracked}
+        self._stage = None
         self.units_by_conv = {id(u.fwd): u for u in T.units.values()}
         self.d_units_by_conv = {id(u.fwd): u for u in E.units.values()}
         self.stats = {}       # tag -> [checks, worst err/tol (or worst error of exact checks), exact?]
@@ -338,11 +433,21 @@ class Lockstep(Harness):
         if self.bn_apply_elems:
             lines.append("bn_apply outputs one fp16 ulp from the correctly rounded value: %d of %d" % (self.ulp_flips, self.bn_apply_elems))
         lines.append("ops checked: %d forward, %d backward" % (len(self.checked["fwd"]), len(self.checked["bwd"])))
+        for fam in ("partial_reduce", "channel_reduce", "final_bwd_dw"):
+            ls_ = [la for la in self.launches if la.family == fam]
+            if ls_:
+                la = max(ls_, key=lambda la: la.chain)
+                lines.append("derived sum bound %-15s longest fp32 chain %4d (%s), e_sum %.3g; %d of %d launches capped" % (
+                    fam, la.chain, la.name, la.e_sum(), sum(x.capped for x in ls_), len(ls_)))
+        lines.append("conv.stats bound gamma_31 = %.3g" % E_CONV_STATS)
         return lines
 
     # ------------------------------------------------------------------ driver
-    def run(self, x, dlogits, raise_on_fail=True, dut_x=None, dut_dlogits=None):
-        """x: fp32 NCHW input (CPU), dlogits: fp32 NCHW logit gradient (CPU); dut_*: the same on the executor's device"""
+    def run(self, x, dlogits, raise_on_fail=True, dut_x=None, dut_dlogits=None, log=None):
+        """x: fp32 NCHW input (CPU), dlogits: fp32 NCHW logit gradient (CPU); dut_*: the same on the executor's device;
+        log: called with a line per op (its time) when given"""
+        import time
+
         self.raise_on_fail = raise_on_fail
         dx = x if dut_x is None else dut_x
         ddl = dlogits if dut_dlogits is None else dut_dlogits
@@ -353,8 +458,11 @@ class Lockstep(Harness):
                     self.checked[which].add(i)
                     continue
                 fin = (lst_d[i + 1], lst_t[i + 1]) if ot[0] == "bn_stats" else None
+                t0 = time.time()
                 self._step(which, i, od, ot, fin, x, dlogits, dx, ddl)
                 self.checked[which].add(i)
+                if log is not None:
+                    log("%s %3d %-12s %-36s %6.2f s" % (which, i, ot[0], self._name(ot), time.time() - t0))
         assert len(self.checked["fwd"]) == len(self.tw.fwd_ops) and len(self.checked["bwd"]) == len(self.tw.bwd_ops)
         return self.failures
 
@@ -369,6 +477,7 @@ class Lockstep(Harness):
         return k
 
     def _step(self, which, i, od, ot, fin, x, dlogits, dx, ddl):
+        self._cur = (which, i)
         writes = self._reference(ot, x, dlogits)
         self.dut.run(od, x=dx, dlogits=ddl)
         if fin is not None:
@@ -395,9 +504,10 @@ class Lockstep(Harness):
                 du = self.d_units_by_conv[id(self._dut_op(which, i)[1])]
                 rows, C = u.stats_rows, u.desc.Cout
                 part = du.stats[:rows * 2 * C].double().cpu().reshape(rows, 2, C).sum(0).numpy()
-                z = _f64(u.out).reshape(-1, C)  # the kernel's own output, already copied into the twin
-                for j, (ref, mag) in enumerate(((z.sum(0), np.abs(z).sum(0)), ((z * z).sum(0), (z * z).sum(0)))):
-                    err, tol = np.abs(part[j] - ref), E_SUM * mag + 1e-30
+                z = self._colsums(u.out, C, lambda z: (z, np.abs(z), z * z))  # the kernel's own output, already copied into the twin
+                e = E_CONV_STATS + rows * 2.0 ** -53
+                for j, (ref, mag) in enumerate(((z[0], z[1]), (z[2], z[2]))):
+                    err, tol = np.abs(part[j] - ref), e * mag + 1e-30
                     st = self.stats.setdefault("conv.stats", [0, 0.0, False])
                     st[0] += 1
                     st[1] = max(st[1], float((err / tol).max()))
@@ -414,6 +524,23 @@ class Lockstep(Harness):
                 self._fail(which, i, ot, b.prefix + ".sums", "accumulator slots / arrival counter not cleared (first nonzero double %d)" % first)
             self.tb[idx].copy_(self.db[idx].cpu())
 
+    def _colsums(self, t, C, terms):
+        """column sums over the rows of (twin) tensor t viewed [M, C] as float64, of each array terms(rows) returns, in chunks"""
+        v = t.reshape(-1, C)
+        step = max(1, self.chunk // C)
+        parts = emulate.pmap(lambda a: [p.sum(0) for p in terms(v[a:a + step].double().numpy())], range(0, v.shape[0], step))
+        return [sum(col) for col in zip(*parts)]
+
+    def _write_lazy(self, label, t, shape, fn, tag):
+        """output = the whole of contiguous (twin) tensor t viewed as `shape`, reference fn(a, b) over rows a:b of it"""
+        i, off = self._locate(t.data_ptr())
+        assert t.is_contiguous() and int(np.prod(shape)) == t.numel()
+        strides = tuple(int(np.prod(shape[k + 1:])) for k in range(len(shape)))
+        return _Write(label, i, off, shape, strides, None, None, tag, fn=fn)
+
+    def _e_sum(self, family):
+        return self.launch[self._cur][family].e_sum()
+
     def _dut_op(self, which, i):
         return (self.dut.eng.fwd_ops if which == "fwd" else self.dut.eng.bwd_ops)[i]
 
@@ -424,21 +551,64 @@ class Lockstep(Harness):
     def _ref_conv(self, op, x, dlogits):
         d = op[1].desc
         K = 64 * sum(d.segs[j].cblocks for j in range(d.nseg))
+        tag = "conv.dgrad" if ".dgrad" in op[1].name else "conv"
         writes = []
+        if self.sample_above is not None and d.mode == 0 and d.phases * d.Nt * d.Ht * d.Wt > self.sample_above:
+            pix = self._conv_sample(d)
+            val, mag, addr = emulate.conv_f64_at(d, pix)
+            tol = ulp16(val) + K * U * mag
+            for phase, base, shape, strides in emulate.conv_out_views(d):
+                sel = pix[:, 3] == phase
+                idx, off = self._locate(base)
+                sample = ((addr[sel] - self.tb[idx].data_ptr()) // 2)[:, None] + np.arange(d.Cout)[None, :]
+                writes.append(_Write("%s out (%s, sampled)" % (op[1].name, self._blabel(idx)), idx, off, shape, strides, val[sel], tol[sel], tag,
+                                     d.out_plane if d.split else 0, sample=sample))
+            return writes
 
         def sink(ptr, shape, strides, val, mag, parts, plane):
             idx, off = self._locate(ptr)
-            tag = "conv.dgrad" if ".dgrad" in op[1].name else "conv"
             writes.append(_Write("%s out (%s)" % (op[1].name, self._blabel(idx)), idx, off, shape, strides, val, ulp16(val) + K * U * mag, tag))
 
         emulate.run_desc(d, sink=sink)
         return writes
 
+    def _rng(self):
+        which, i = self._cur
+        return np.random.default_rng([self.seed, 0 if which == "fwd" else 1, i])
+
+    def _conv_sample(self, d):
+        """sampled output pixels of descriptor d, [S, 4] (n, y, x, phase): for every image the whole first, last and one seeded
+        random tile box of the kernel's TW x TH x TN tiling (the random box is shared by the TN images of a box), the four
+        corners and 256 seeded random pixels; every phase of each"""
+        rng = self._rng()
+        nbw, nbh, nbn = -(-d.Wt // d.TW), -(-d.Ht // d.TH), -(-d.Nt // d.TN)
+        rand_box = [(int(rng.integers(nbw)), int(rng.integers(nbh))) for _ in range(nbn)]
+        pts = []
+        for n in range(d.Nt):
+            for bx, by in ((0, 0), (nbw - 1, nbh - 1), rand_box[n // d.TN]):
+                yy, xx = np.meshgrid(np.arange(by * d.TH, min(d.Ht, (by + 1) * d.TH)), np.arange(bx * d.TW, min(d.Wt, (bx + 1) * d.TW)), indexing="ij")
+                pts.append(np.stack([np.full(yy.size, n), yy.reshape(-1), xx.reshape(-1)], 1))
+            pts.append(np.array([[n, 0, 0], [n, 0, d.Wt - 1], [n, d.Ht - 1, 0], [n, d.Ht - 1, d.Wt - 1]]))
+            pts.append(np.stack([np.full(256, n), rng.integers(d.Ht, size=256), rng.integers(d.Wt, size=256)], 1))
+        pix = np.unique(np.concatenate(pts).astype(np.int64), axis=0)
+        return np.concatenate([np.concatenate([pix, np.full((len(pix), 1), ph, np.int64)], 1) for ph in range(d.phases)])
+
     def _ref_wgrad(self, op, x, dlogits):
         _, u, dy = op
         d = u.desc
-        ref, mag = emulate.run_wgrad(d, dy.data_ptr() + 2 * u.out_offset, None, f64=True)
         P = d.Nt * d.Ht * d.Wt
+        ptr = dy.data_ptr() + 2 * u.out_offset
+        if self.sample_above is not None and d.phases * P > self.sample_above:
+            R = d.phases * d.Cout
+            K = 64 * sum(d.segs[j].cblocks for j in range(d.nseg))
+            rows = {r for r in (0, 63, 64, 127, 128, R - 1) if r < R} | {int(r) for r in self._rng().choice(R, min(4, R), replace=False)}
+            rows = np.array(sorted(rows), dtype=np.int64)
+            ref, mag = emulate.run_wgrad_rows(d, ptr, rows)
+            idx, off = self._locate(u.dw_packed.data_ptr())
+            sample = off + rows[:, None] * K + np.arange(K)[None, :]
+            return [_Write(u.name + ".dw_packed (sampled rows)", idx, off, u.dw_packed.shape, u.dw_packed.stride(), ref,
+                           2.0 ** -23 * (P / 16 + P / 64 + 17) * mag, "wgrad", sample=sample)]
+        ref, mag = emulate.run_wgrad(d, ptr, None, f64=True)
         tol = 2.0 ** -23 * (P / 16 + P / 64 + 17) * mag
         return [self._write_t(u.name + ".dw_packed", u.dw_packed, ref, tol, "wgrad")]
 
@@ -449,10 +619,10 @@ class Lockstep(Harness):
     def _ref_bn_stats(self, op, x, dlogits):
         b = op[1]
         P = self.tw.params
-        z = _f64(b.z).reshape(b.M, b.C)
+        s1, sa, s2 = self._colsums(b.z, b.C, lambda z: (z, np.abs(z), z * z))
         M = float(b.M)
-        mean = z.sum(0) / M
-        ez2 = (z * z).sum(0) / M
+        mean = s1 / M
+        ez2 = s2 / M
         var = np.maximum(ez2 - mean * mean, 0)
         invstd = 1.0 / np.sqrt(var + BN_EPS)
         gamma, beta = self._bn_params(b)
@@ -460,8 +630,9 @@ class Lockstep(Harness):
         shift = beta - mean * scale
         rm, rv = _f64(P[b.prefix + ".running_mean"]), _f64(P[b.prefix + ".running_var"])
         unb = var * M / (M - 1) if M > 1 else var
-        d_mean = E_SUM * np.abs(z).sum(0) / M + U * np.abs(mean)
-        d_var = E_SUM * ez2 + 2 * np.abs(mean) * d_mean
+        e_s = self._e_sum("partial_reduce")
+        d_mean = e_s * sa / M + U * np.abs(mean)
+        d_var = e_s * ez2 + 2 * np.abs(mean) * d_mean
         d_inv = invstd * (d_var / (2 * (var + BN_EPS)) + 2 * U)
         d_scale = np.abs(gamma) * d_inv + U * np.abs(scale)
         d_shift = np.abs(mean) * d_scale + np.abs(scale) * d_mean + 2 * U * (np.abs(beta) + np.abs(mean * scale))
@@ -480,65 +651,101 @@ class Lockstep(Harness):
 
     def _ref_bn_apply(self, op, x, dlogits):
         _, b, res, y, relu = op
-        z = _f64(b.z).reshape(b.M, b.C)
+        C = b.C
         sc, sh = _f64(b.scale), _f64(b.shift)
-        o = z * sc + sh
-        mag = np.abs(z * sc) + np.abs(sh)
-        if res is not None:
-            r = _f64(res).reshape(b.M, b.C)
-            o = o + r
-            mag = mag + np.abs(r)
-        if relu:
-            o = np.maximum(o, 0)
-        return [self._write_t(b.prefix + " y", y, o, ulp16(o) + 2.0 ** -23 * mag, "bn_apply")]
+        zv = b.z.reshape(-1, C)
+        rv = res.reshape(-1, C) if res is not None else None
+
+        def fn(a, e):
+            z = zv[a:e].double().numpy()
+            o = z * sc + sh
+            mag = np.abs(z * sc) + np.abs(sh)
+            if rv is not None:
+                r = rv[a:e].double().numpy()
+                o = o + r
+                mag = mag + np.abs(r)
+            if relu:
+                o = np.maximum(o, 0)
+            return o, ulp16(o) + 2.0 ** -23 * mag
+
+        return [self._write_lazy(b.prefix + " y", y, (b.M, C), fn, "bn_apply")]
 
     def _ref_bn_bwd(self, op, x, dlogits):
         _, b, dy, y, dz, g_out = op
         M, C = b.M, b.C
-        g = _f64(dy).reshape(M, C)
-        if y is not None:
-            g = g * (_f64(y).reshape(M, C) > 0)
-        z = _f64(b.z).reshape(M, C)
         mu, inv = _f64(b.mean), _f64(b.invstd)
+        dyv, yv, zv = dy.reshape(M, C), (y.reshape(M, C) if y is not None else None), b.z.reshape(M, C)
+
+        def g_of(a, e):
+            g = dyv[a:e].double().numpy()
+            return g * (yv[a:e].double().numpy() > 0) if yv is not None else g
+
+        def part(a):
+            g, z = g_of(a, a + step), zv[a:a + step].double().numpy()
+            return [p.sum(0) for p in (g, g * ((z - mu) * inv), np.abs(g), np.abs(g * z))]
+
+        step = max(1, self.chunk // C)
+        s0, s1, sg, sgz = [sum(col) for col in zip(*emulate.pmap(part, range(0, M, step)))]
         gamma, _ = self._bn_params(b)
-        zh = (z - mu) * inv
-        s0, s1 = g.sum(0), (g * zh).sum(0)
         A = gamma * inv
         Bc = -gamma * inv * inv * s1 / M
         D = -gamma * inv * s0 / M + gamma * inv * inv * mu * s1 / M
-        ref = A * g + Bc * z + D
-        d_s0 = E_SUM * np.abs(g).sum(0)
-        d_s1 = E_SUM * inv * (np.abs(g * z).sum(0) + np.abs(mu) * np.abs(g).sum(0))
-        tol = ulp16(ref) + 2.0 ** -22 * (np.abs(A * g) + np.abs(Bc * z) + np.abs(D)) + np.abs(A) * (d_s0 + np.abs(zh) * d_s1) / M
+        e_s = self._e_sum("channel_reduce")
+        d_s0 = e_s * sg
+        d_s1 = e_s * inv * (sgz + np.abs(mu) * sg)
+
+        def fn_dz(a, e):
+            g, z = g_of(a, e), zv[a:e].double().numpy()
+            zh = (z - mu) * inv
+            ref = A * g + Bc * z + D
+            return ref, ulp16(ref) + 2.0 ** -22 * (np.abs(A * g) + np.abs(Bc * z) + np.abs(D)) + np.abs(A) * (d_s0 + np.abs(zh) * d_s1) / M
+
         ls = float(self.tw.loss_scale)
-        out = [self._write_t(b.prefix + " dz", dz, ref, tol, "bn_bwd.dz")]
+        out = [self._write_lazy(b.prefix + " dz", dz, (M, C), fn_dz, "bn_bwd.dz")]
         if g_out is not None:
-            out.append(self._write_t(b.prefix + " g_out", g_out, g, 0.0, "bn_bwd.g_out"))
+            out.append(self._write_lazy(b.prefix + " g_out", g_out, (M, C), lambda a, e: (g_of(a, e), 0.0), "bn_bwd.g_out"))
         out.append(self._write_t(b.prefix + ".weight grad", self.tw.grads[b.prefix + ".weight"], s1 / ls, d_s1 / ls + 2 * U * np.abs(s1 / ls), "bn_bwd.dgamma_dbeta"))
         out.append(self._write_t(b.prefix + ".bias grad", self.tw.grads[b.prefix + ".bias"], s0 / ls, d_s0 / ls + 2 * U * np.abs(s0 / ls), "bn_bwd.dgamma_dbeta"))
         return out
 
     def _ref_relu_bwd(self, op, x, dlogits):
-        _, a, b2, y, out = op
-        s = a.float()
-        if b2 is not None:
-            s = s + b2.float()
-        if y is not None:
-            s = s * (y.float() > 0)
-        return [self._write_t("relu_bwd out", out, _f64(s.half()), 0.0, "relu_bwd")]
+        _, a_, b2, y, out = op
+        C = out.shape[-1]
+        av, bv, yv = a_.reshape(-1, C), (b2.reshape(-1, C) if b2 is not None else None), (y.reshape(-1, C) if y is not None else None)
+
+        def fn(a, e):
+            s = av[a:e].float()
+            if bv is not None:
+                s = s + bv[a:e].float()
+            if yv is not None:
+                s = s * (yv[a:e].float() > 0)
+            return _f64(s.half()), 0.0
+
+        return [self._write_lazy("relu_bwd out", out, (out.numel() // C, C), fn, "relu_bwd")]
 
     def _ref_maxpool(self, op, x, dlogits):
         _, src, dst, n, h, w, c, kk, s, p = op
-        yy = F.max_pool2d(src.double().reshape(n, h, w, c).permute(0, 3, 1, 2), kk, s, p).permute(0, 2, 3, 1)
-        return [self._write_t("maxpool out", dst, yy.numpy(), 0.0, "maxpool")]
+        sv = src.reshape(n, h, w, c)
+
+        def fn(a, e):
+            return F.max_pool2d(sv[a:e].double().permute(0, 3, 1, 2), kk, s, p).permute(0, 2, 3, 1).numpy(), 0.0
+
+        return [self._write_lazy("maxpool out", dst, tuple(dst.shape), fn, "maxpool")]
 
     def _ref_maxpool_bwd(self, op, x, dlogits):
         _, xx, dy, dx, n, h, w, c, kk, s, p = op
-        xin = xx.double().reshape(n, h, w, c).permute(0, 3, 1, 2).clone().requires_grad_(True)
-        yy = F.max_pool2d(xin, kk, s, p)
-        yy.backward(dy.double().reshape(n, yy.shape[2], yy.shape[3], c).permute(0, 3, 1, 2))
-        ref = xin.grad.permute(0, 2, 3, 1).numpy()
-        return [self._write_t("maxpool_bwd dx", dx, ref, ulp16(ref), "maxpool_bwd")]
+        xv = xx.reshape(n, h, w, c)
+        oh, ow = (h + 2 * p - kk) // s + 1, (w + 2 * p - kk) // s + 1
+        dyv = dy.reshape(n, oh, ow, c)
+
+        def fn(a, e):
+            xin = xv[a:e].double().permute(0, 3, 1, 2).clone().requires_grad_(True)
+            yy = F.max_pool2d(xin, kk, s, p)
+            yy.backward(dyv[a:e].double().permute(0, 3, 1, 2))
+            ref = xin.grad.permute(0, 2, 3, 1).numpy()
+            return ref, ulp16(ref)
+
+        return [self._write_lazy("maxpool_bwd dx", dx, (n, h, w, c), fn, "maxpool_bwd")]
 
     def _ref_prepass(self, op, x, dlogits):
         return [self._write_t("s2d", self.tw.s2d, _f64(emulate.prepass_s2d_cpu(x)), 0.0, "prepass")]
@@ -586,29 +793,38 @@ class Lockstep(Harness):
     def _ref_final_fwd(self, op, x, dlogits):
         _, y5, logits = op
         P = self.tw.params
-        y = _f64(y5)  # [N, H, W, 32]
         w = _f64(P["final.weight"]).reshape(self.tw.C, 32)
         b = _f64(P["final.bias"])
-        ref = np.einsum("nhwc,kc->nkhw", y, w) + b[None, :, None, None]
-        mag = np.einsum("nhwc,kc->nkhw", np.abs(y), np.abs(w)) + np.abs(b)[None, :, None, None]
-        return [self._write_t("logits", logits, ref, 34 * U * mag, "final_fwd")]
+
+        def fn(a, e):
+            y = y5[a:e].double().numpy()  # [n, H, W, 32]
+            ref = np.einsum("nhwc,kc->nkhw", y, w) + b[None, :, None, None]
+            mag = np.einsum("nhwc,kc->nkhw", np.abs(y), np.abs(w)) + np.abs(b)[None, :, None, None]
+            return ref, 34 * U * mag
+
+        return [self._write_lazy("logits", logits, tuple(logits.shape), fn, "final_fwd")]
 
     def _ref_final_bwd(self, op, x, dlogits):
         _, y5, d_y5 = op
         T = self.tw
         w = _f64(T.params["final.weight"]).reshape(T.C, 32)
-        dl = dlogits.double().numpy()
-        y = _f64(y5)
         ls = float(T.loss_scale)
-        d = np.einsum("nkhw,kc->nhwc", dl, w) * ls
-        dmag = np.einsum("nkhw,kc->nhwc", np.abs(dl), np.abs(w)) * ls
-        dw = np.einsum("nkhw,nhwc->kc", dl, y)
-        dwm = np.einsum("nkhw,nhwc->kc", np.abs(dl), np.abs(y))
-        db, dbm = dl.sum((0, 2, 3)), np.abs(dl).sum((0, 2, 3))
-        return [self._write_t("d_y5", d_y5, d, ulp16(d) + (T.C + 2) * U * dmag, "final_bwd.dy5"),
-                self._write_t("final.weight grad", T.grads["final.weight"], dw, E_SUM * dwm + 2 * U * np.abs(dw), "final_bwd.dw_db"),
-                self._write_t("final.bias grad", T.grads["final.bias"], db, E_SUM * dbm + 2 * U * np.abs(db), "final_bwd.dw_db")]
+        def part(n):  # one image: [classes, HW] x [HW, 32]
+            dl, y = dlogits[n].double().numpy().reshape(T.C, -1), y5[n].double().numpy().reshape(-1, 32)
+            return dl @ y, np.abs(dl) @ np.abs(y), dl.sum(1), np.abs(dl).sum(1)
 
+        dw, dwm, db, dbm = [sum(col) for col in zip(*emulate.pmap(part, range(y5.shape[0])))]
+
+        def fn(a, e):
+            dl = dlogits[a:e].double().numpy()
+            d = np.einsum("nkhw,kc->nhwc", dl, w) * ls
+            dmag = np.einsum("nkhw,kc->nhwc", np.abs(dl), np.abs(w)) * ls
+            return d, ulp16(d) + (T.C + 2) * U * dmag
+
+        e_s = self._e_sum("final_bwd_dw")
+        return [self._write_lazy("d_y5", d_y5, tuple(d_y5.shape), fn, "final_bwd.dy5"),
+                self._write_t("final.weight grad", T.grads["final.weight"], dw, e_s * dwm + 2 * U * np.abs(dw), "final_bwd.dw_db"),
+                self._write_t("final.bias grad", T.grads["final.bias"], db, e_s * dbm + 2 * U * np.abs(db), "final_bwd.dw_db")]
 
 
 def make_pair(C, B, H, W, loss_scale, device, seed=0):

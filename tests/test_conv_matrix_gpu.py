@@ -11,7 +11,7 @@ Per case:
     and the one-CTA schedules give the same bits too;
   * rsb_conv_plan_info: tiles, K blocks, grid and shared memory as the descriptor implies;
   * statistics instances: every per-quarter-tile partial equals the float64 sums of the stored fp16 outputs of its 32 rows
-    (ragged rows excluded) within lockstep.py's E_SUM.
+    (ragged rows excluded) within lockstep.py's E_CONV_STATS (31 fp32 roundings).
 """
 
 import ctypes
@@ -22,7 +22,7 @@ import torch
 
 import conv_matrix as CM
 import emulate
-from lockstep import E_SUM
+from lockstep import E_CONV_STATS
 from predict_lockstep import conv_tol
 from robosat_b200 import _lib
 from robosat_b200._lib import RowConvDesc
@@ -107,7 +107,7 @@ def _check_stats(case, d, got_out, got_stats, meta):
     mag = torch.stack([torch.zeros(rows, C, dtype=torch.float64).index_add_(0, q, zf.abs()), ref[1]])
     part = got_stats[:rows * 2 * C].double().reshape(rows, 2, C).permute(1, 0, 2)
     err = (part - ref).abs()
-    tol = E_SUM * mag + 1e-30
+    tol = E_CONV_STATS * mag + 1e-30
     bad = ~(err <= tol)
     assert not bad.any(), "%s: %d statistics partial(s) off, first at (sum|sq, quarter row, channel) %s: %r vs %r" % (
         case.name, int(bad.sum()), tuple(torch.nonzero(bad)[0].tolist()), float(part[bad][0]), float(ref[bad][0]))
