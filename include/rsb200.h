@@ -633,6 +633,17 @@ int rsb_tiff_decode_window(const uint8_t* file_host, int64_t file_len, const int
                            int32_t compression, int32_t predictor, int64_t row0, int64_t rows, int64_t col0, int64_t cols, uint8_t* out_host,
                            int32_t threads, int64_t* bad_chunk_host);
 
+/* The band rule (DESIGN.md §8): decode raster rows [row0, row0 + rows) x columns [col0, col0 + cols) of an uncompressed, LZW or
+ * DEFLATE TIFF of spp samples per pixel, bits 8 or 16 each, into out_host [rows][cols][k]: sample j of a pixel is band
+ * select_host[j] (0-based, 1 <= k <= 4), uint8 or native-endian uint16. planar 1: chunky chunks as rsb_tiff_decode_window;
+ * planar 2: num_chunks holds spp planes of chunks, band after band, and only the selected bands' chunks are read. big_endian: the
+ * file's byte order. predictor 2 undoes horizontal differencing on whole samples, modulo 2^bits, after the byte-order conversion.
+ * Errors as rsb_tiff_decode_window (the bad chunk's index counts the planes before it). Host only: no device needed. */
+int rsb_tiff_decode_bands(const uint8_t* file_host, int64_t file_len, const int64_t* chunk_offsets_host, const int64_t* chunk_bytes_host,
+                          int64_t num_chunks, int64_t width, int64_t height, int32_t chunk_w, int32_t chunk_h, int32_t tiled, int32_t spp,
+                          int32_t bits, int32_t planar, int32_t big_endian, int32_t compression, int32_t predictor, const int32_t* select_host,
+                          int32_t k, int64_t row0, int64_t rows, int64_t col0, int64_t cols, void* out_host, int32_t threads, int64_t* bad_chunk_host);
+
 /* JPEG (Compression 7) strips or tiles (DESIGN.md §8). Parse JPEGTables (tables_host [tables_len], tables_len 0 when absent) and
  * the headers of the chunks select_host [num_select] (NULL: all num_chunks chunks, in order) of file_host (chunk_offsets_host,
  * chunk_bytes_host, the raster and chunk sizes as rsb_tiff_decode_window; rows_per_strip is the TIFF's RowsPerStrip, at least
@@ -700,6 +711,19 @@ int rsb_tile_average(const uint8_t* src, int64_t src_pitch, int64_t win_row0, in
                      int64_t raster_w, int64_t raster_h, int32_t spp, int32_t alpha, int32_t nodata, const double* nodes, int64_t node_x0,
                      int64_t node_y0, int32_t nodes_w, int32_t nodes_h, int32_t grid_step, const int64_t* tiles, int32_t N, int32_t size,
                      uint8_t* out, int64_t image_stride, int64_t* covered, int64_t* misses, void* stream);
+
+/* The band rule (DESIGN.md §8). src [rows][cols][nsel + alpha] samples of `bits` (8: uint8, 16: uint16), 16-byte aligned: nsel (1
+ * or 3) selected bands, then the alpha band when alpha = 1. A pixel is invalid when its alpha sample is 0 or every selected band
+ * equals nodata (-1: none; else 0 .. 2^bits - 1). rsb_tile_render writes out uint8 [rows][out_pitch] (4-byte aligned, out_pitch a
+ * multiple of 4 and at least 4 cols): per pixel R, G, B, A with band b's value v = floor((510 t + d) / (2 d)), d = HI - LO,
+ * t = clamp(s, LO, HI) - LO for scale_host int32 [nsel][2] = (LO, HI), 0 <= LO < HI <= 2^bits - 1 (one band: R = G = B = v), and
+ * A = 0 for an invalid pixel, else 255; the input rsb_tile_warp and rsb_tile_average take with spp 4, alpha 1, nodata -1.
+ * rsb_band_histogram adds the count of every value of each selected band over the valid pixels to hist int64 [nsel][2^bits], which
+ * it does not clear. Arguments are validated before the device check; neither allocates nor synchronises. */
+int rsb_tile_render(const void* src, int64_t rows, int64_t cols, int32_t bits, int32_t nsel, int32_t alpha, int32_t nodata, const int32_t* scale_host,
+                    uint8_t* out, int64_t out_pitch, void* stream);
+int rsb_band_histogram(const void* src, int64_t rows, int64_t cols, int32_t bits, int32_t nsel, int32_t alpha, int32_t nodata, int64_t* hist,
+                       void* stream);
 
 /* rs mosaic (DESIGN.md §8): deflate the chunk x chunk tiles of one row of a 1-band 8-bit raster window. window_host uint8 rows x cols
  * (row pitch `pitch`, rows <= chunk); tile k holds columns [k chunk, (k + 1) chunk) and is padded with `fill` past the window's rows

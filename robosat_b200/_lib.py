@@ -254,6 +254,8 @@ SIGNATURES = {
     "rsb_png_write_rgb8_batch": (ctypes.c_int, [_vp, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _i32]),
     "rsb_tiff_decode_window": (ctypes.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64,
                                               _vp, _i32, _vp]),
+    "rsb_tiff_decode_bands": (ctypes.c_int, [_vp, _i64, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _i32,
+                                             _i64, _i64, _i64, _i64, _vp, _i32, _vp]),
     "rsb_jpeg_parse_chunks": (ctypes.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i64, _i32, _i32, _i32, _vp, _i64, _i32,
                                              _vp, _vp, _i32, _vp, _vp]),
     "rsb_jpeg_scratch_bytes": (_i64, [_i64]),
@@ -263,6 +265,8 @@ SIGNATURES = {
                                      _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
     "rsb_tile_average": (ctypes.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _vp,
                                         _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
+    "rsb_tile_render": (ctypes.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
+    "rsb_band_histogram": (ctypes.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     "rsb_tiff_deflate_bound": (_i64, [_i64]),
     "rsb_tiff_encode_chunks": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i32]),
     "rsb_mosaic_warp": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _i64, _i32, _i32, _i32, _i64, _i64,

@@ -5,7 +5,7 @@ cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xptxas -v --expt-relaxed-constexpr"
 OBJS=""
-for f in rsb_host rsb_conv rsb_conv_row rsb_elementwise rsb_loss rsb_train rsb_wgrad rsb_morph rsb_label rsb_raster rsb_cover rsb_dedupe rsb_merge rsb_extract rsb_compare rsb_tile rsb_mosaic rsb_road rsb_jpeg; do
+for f in rsb_host rsb_conv rsb_conv_row rsb_elementwise rsb_loss rsb_train rsb_wgrad rsb_morph rsb_label rsb_raster rsb_cover rsb_dedupe rsb_merge rsb_extract rsb_compare rsb_tile rsb_bands rsb_mosaic rsb_road rsb_jpeg; do
   $NVCC $FLAGS -c $f.cu -o $f.o 2> $f.ptxas.log || { cat $f.ptxas.log; exit 1; }
   OBJS="$OBJS $f.o"
 done

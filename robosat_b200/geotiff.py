@@ -8,6 +8,10 @@ a pixel scale or by an affine model transformation, in EPSG:3857, EPSG:4326 or a
 Anything else raises `RsbError` naming the value found. Overviews and sub-IFDs are ignored. `read_window` decodes a window of rows
 and columns with the library's decoder (`rsb_tiff_decode_window`) over a memory map of the file, or for JPEG on the device.
 
+`open_bands(path, bands)` reads the same container under the band rule of `rs tile --bands / --scale / --stretch` (DESIGN.md §8):
+8- or 16-bit unsigned samples, chunky or planar, MinIsBlack or RGB with any number of bands, 1 or 3 of them selected plus the alpha
+band, decoded by `rsb_tiff_decode_bands`. `GeoTiff(path)` keeps its own rule and messages.
+
 `read_grid(path)` reads only the size and the georeferencing, with the same rules and messages for those, so any pixel layout
 (16-bit, JPEG, palette ...) is accepted: `rs mosaic --like` takes the grid of an existing raster.
 """
@@ -274,6 +278,12 @@ class GeoTiff(_Header):
             _fail(self.path, "Predictor %d is not supported; use 1 or 2" % self.predictor)
         if self.compression in (1, JPEG):
             self.predictor = 1  # libtiff applies the predictor only inside a codec other than JPEG; uncompressed data is stored as is
+        self._chunk_table(1)
+        self.nodata = self._nodata(255)
+
+    def _chunk_table(self, planes):
+        """tiled, chunk_w, chunk_h, rows_per_strip and the offsets / byte_counts of `planes` planes of chunks"""
+        t = self._tag
         if 322 in self._tags:
             self.tiled = True
             self.chunk_w, self.chunk_h = int(t(322)[0]), int(t(323, (0,))[0])
@@ -286,6 +296,7 @@ class GeoTiff(_Header):
             self.chunk_w, self.chunk_h = self.width, min(self.height, self.rows_per_strip)
             offsets, counts = t(273), t(279)
             need = -(-self.height // max(1, self.chunk_h))
+        need *= planes
         if self.chunk_w < 1 or self.chunk_h < 1:
             _fail(self.path, "chunks of %d x %d pixels" % (self.chunk_w, self.chunk_h))
         if offsets is None or counts is None or len(offsets) != need or len(counts) != need:
@@ -293,15 +304,18 @@ class GeoTiff(_Header):
                 "tile" if self.tiled else "strip", None if offsets is None else len(offsets), None if counts is None else len(counts), need))
         self.offsets = np.asarray(offsets, np.int64)
         self.byte_counts = np.asarray(counts, np.int64)
+
+    def _nodata(self, top):
+        """the integer value of GDAL_NODATA in 0..top, or -1 (any other value matches no pixel)"""
         nodata = self._tags.get(42113)
-        self.nodata = -1
         if nodata:
             try:
                 value = float(nodata.strip())
             except ValueError:
                 _fail(self.path, "GDAL_NODATA %r is not a number" % nodata)
-            if math.isfinite(value) and value == int(value) and 0 <= value <= 255:  # any other value matches no 8-bit pixel
-                self.nodata = int(value)
+            if math.isfinite(value) and value == int(value) and 0 <= value <= top:
+                return int(value)
+        return -1
 
     # ---- pixels ----
 
@@ -330,6 +344,127 @@ class GeoTiff(_Header):
                                                        self.spp, self.compression, self.predictor, row0, rows, col0, cols, view.ctypes.data,
                                                        threads or usable_cores(), ctypes.byref(bad)), "%s" % self.path)
         return view.reshape(rows, cols, self.spp)
+
+
+
+def open_bands(path, bands=None):
+    """IFD 0 of a GeoTIFF read under the band rule (DESIGN.md §8; `rs tile --bands / --scale / --stretch`): a `BandTiff` whose window
+    decode gathers the 1-based `bands` (1 or 3 of them; None: 1,2,3 of an RGB raster, or the band of a single MinIsBlack band with or
+    without an alpha band) and the alpha band"""
+    return BandTiff(path, bands)
+
+
+class BandTiff(GeoTiff):
+    """A GeoTiff under the band rule. Besides GeoTiff's attributes (spp is the file's samples per pixel, nodata is in 0..2^bits - 1 or
+    -1): bits (8 or 16), planar (1 chunky, 2 band-interleaved), byteorder ('<' or '>'), bands (the 0-based selected bands, 1 or 3),
+    alpha_band (0-based, or None: the first band ExtraSamples declares alpha), k (the decoded samples per pixel: the selected bands,
+    then the alpha band), and scale: [(LO, HI)] per selected band, the identity (0, 255) for 8-bit rasters and None for 16-bit
+    ones until set (`set_scale`)."""
+
+    def __init__(self, path, bands=None):
+        self._want = None if bands is None else [int(b) for b in bands]
+        super().__init__(path)
+
+    def _parse(self):
+        self._parse_tags()
+        self._size()
+        self._band_image()
+        self._georeference()
+
+    def _band_image(self):
+        t = self._tag
+        self.compression = int(t(259, (1,))[0])
+        if self.compression not in COMPRESSIONS or self.compression == JPEG:
+            _fail(self.path, "Compression %d (%s) is not supported with --bands, --scale or --stretch; use none, LZW or deflate" % (
+                self.compression, COMPRESSION_NAMES.get(self.compression, "unknown")))
+        self.spp = int(t(277, (1,))[0])
+        if self.spp < 1:
+            _fail(self.path, "SamplesPerPixel %d" % self.spp)
+        bits = tuple(int(b) for b in t(258, (1,) * self.spp))
+        if len(set(bits)) != 1 or bits[0] not in (8, 16):
+            _fail(self.path, "BitsPerSample %s is not supported; use 8 or 16 for every band" % ",".join(str(b) for b in bits))
+        self.bits = bits[0]
+        fmt = t(339, (1,) * self.spp)
+        if any(int(f) != 1 for f in fmt):
+            _fail(self.path, "SampleFormat %s is not supported; only 1 (unsigned integer) is" % (",".join(str(int(f)) for f in fmt)))
+        self.planar = int(t(284, (1,))[0])
+        if self.planar not in (1, 2):
+            _fail(self.path, "PlanarConfiguration %d is not supported; use 1 (chunky) or 2 (planar)" % self.planar)
+        self.photometric = int(t(262, (1 if self.spp < 3 else 2,))[0])
+        if self.photometric not in (1, 2):
+            _fail(self.path, "Photometric %d (%s) is not supported; use MinIsBlack or RGB" % (
+                self.photometric, PHOTOMETRIC_NAMES.get(self.photometric, "unknown")))
+        if self.photometric == 2 and self.spp < 3:
+            _fail(self.path, "Photometric 2 (RGB) with %d bands" % self.spp)
+        extra = tuple(int(v) for v in t(338, ()))
+        if len(extra) > self.spp:
+            _fail(self.path, "ExtraSamples has %d values for %d bands" % (len(extra), self.spp))
+        first_extra = self.spp - len(extra)
+        self.alpha_band = next((first_extra + i for i, v in enumerate(extra) if v in (1, 2)), None)
+        if self._want is None:
+            if self.photometric == 2:
+                self.bands = [0, 1, 2]
+            elif self.spp == 1 or (self.spp == 2 and self.alpha_band == 1):
+                self.bands = [0]
+            else:
+                _fail(self.path, "%d bands (Photometric %s) need --bands to say which to read" % (
+                    self.spp, PHOTOMETRIC_NAMES[self.photometric]))
+        else:
+            if len(self._want) not in (1, 3):
+                _fail(self.path, "--bands takes 1 or 3 bands, not %d" % len(self._want))
+            for b in self._want:
+                if not 1 <= b <= self.spp:
+                    _fail(self.path, "band %d is not in this raster of %d bands" % (b, self.spp))
+            self.bands = [b - 1 for b in self._want]
+        self.alpha = self.alpha_band is not None
+        self.k = len(self.bands) + int(self.alpha)
+        self.predictor = int(t(317, (1,))[0])
+        if self.predictor not in (1, 2):
+            _fail(self.path, "Predictor %d is not supported; use 1 or 2" % self.predictor)
+        if self.compression == 1:
+            self.predictor = 1  # libtiff applies the predictor only inside a codec; uncompressed data is stored as is
+        self._chunk_table(self.planar == 2 and self.spp or 1)
+        self.nodata = self._nodata((1 << self.bits) - 1)
+        self.scale = [(0, 255)] * len(self.bands) if self.bits == 8 else None
+
+    def set_scale(self, pairs):
+        """the (LO, HI) of every selected band (one pair: the same for all), 0 <= LO < HI <= 2^bits - 1; RsbError otherwise"""
+        pairs = [tuple(int(v) for v in p) for p in pairs]
+        if len(pairs) == 1:
+            pairs = pairs * len(self.bands)
+        if len(pairs) != len(self.bands):
+            raise _lib.RsbError("--scale has %d pairs for %d bands; give one pair, or one per band" % (len(pairs), len(self.bands)))
+        top = (1 << self.bits) - 1
+        for lo, hi in pairs:
+            if not 0 <= lo < hi <= top:
+                raise _lib.RsbError("--scale %d,%d is not 0 <= LO < HI <= %d (%d-bit samples)" % (lo, hi, top, self.bits))
+        self.scale = pairs
+
+    @property
+    def sample_bytes(self):
+        return self.bits // 8
+
+    def read_window(self, row0, rows, col0, cols, out=None, threads=None):
+        """raster rows [row0, row0 + rows) x columns [col0, col0 + cols) -> uint8 or uint16 [rows, cols, k]: the selected bands,
+        then the alpha band (into `out` when given, any C-contiguous array of at least that many bytes, e.g. pinned host memory)"""
+        import ctypes
+
+        from robosat_b200.hostinfo import usable_cores
+
+        dtype = np.uint8 if self.bits == 8 else np.uint16
+        nbytes = rows * cols * self.k * self.sample_bytes
+        if out is None:
+            out = np.empty(nbytes, np.uint8)
+        view = np.frombuffer(out, np.uint8, nbytes) if not isinstance(out, np.ndarray) else out.reshape(-1).view(np.uint8)[:nbytes]
+        select = np.asarray(self.bands + ([self.alpha_band] if self.alpha else []), np.int32)
+        self.file_bytes()
+        bad = ctypes.c_int64(-1)
+        _lib.check(_lib.load().rsb_tiff_decode_bands(self._buf.ctypes.data, self.file_len, self.offsets.ctypes.data, self.byte_counts.ctypes.data,
+                                                      len(self.offsets), self.width, self.height, self.chunk_w, self.chunk_h, int(self.tiled),
+                                                      self.spp, self.bits, self.planar, int(self.byteorder == ">"), self.compression,
+                                                      self.predictor, select.ctypes.data, len(select), row0, rows, col0, cols, view.ctypes.data,
+                                                      threads or usable_cores(), ctypes.byref(bad)), "%s" % self.path)
+        return view.view(dtype).reshape(rows, cols, self.k)
 
 
 def read_grid(path):

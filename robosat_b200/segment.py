@@ -55,7 +55,8 @@ class Plan:
                 store holds indices [img_lo, img_hi) and the plane store [pl_lo, pl_hi) while the op runs
     wait        {k: batch}: warp k overwrites slots whose last reader was that batch's stitch (absent: no earlier reader)
     image_slots, plane_slots, store_bytes: the peaks and what the two stores take (for a JPEG raster, store_bytes also holds
-                decode_bytes: the staged bytes and decoder scratch of the largest warp window)
+                decode_bytes: the staged bytes and decoder scratch of the largest warp window; for a band raster, render_bytes:
+                the raw and the RGBA window buffers, each sized for the largest warp window)
     """
 
 
@@ -108,6 +109,13 @@ def plan(raster, grid, zoom, size, batch=DEFAULT_BATCH, tiles=None, budget=DEFAU
             raise _lib.RsbError("the image and plane stores and the JPEG decode need %d device bytes at their peak (%d tiles of %d x %d x 3, %d of "
                                 "%d x %d and %d bytes of staged chunks and decoder scratch), more than the budget of %d bytes; segment fewer tiles at "
                                 "once with --tiles" % (p.store_bytes, p.image_slots, size, size, p.plane_slots, size, size, p.decode_bytes, budget))
+    if T.is_bands(raster):  # the raw and the RGBA window buffers count too
+        p.render_bytes = max([T.raw_bytes(raster, w.rows, w.cols) for w in p.warps], default=0) + max([w.rows * w.cols * 4 for w in p.warps], default=0)
+        p.store_bytes += p.render_bytes
+        if p.store_bytes > budget:
+            raise _lib.RsbError("the image and plane stores and the band windows need %d device bytes at their peak (%d tiles of %d x %d x 3, %d of "
+                                "%d x %d and %d bytes of raw and RGBA windows), more than the budget of %d bytes; segment fewer tiles at once with "
+                                "--tiles" % (p.store_bytes, p.image_slots, size, size, p.plane_slots, size, size, p.render_bytes, budget))
     if p.store_bytes > budget:
         raise _lib.RsbError("the image and plane stores need %d device bytes at their peak (%d tiles of %d x %d x 3 and %d of %d x %d), more than "
                             "the budget of %d bytes; segment fewer tiles at once with --tiles" % (
@@ -187,7 +195,8 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
     called on a writer thread for every output window, in schedule order, with pixels uint8 [rows, cols] (None: every pixel is
     nodata). Returns the number of existing tiles. `stats`, a dict, receives the counts and the seconds of decode, warp, predict
     (stitch, network, head and vote) and mosaic warp, the last three from CUDA events. For a JPEG raster, decode is the staging of the
-    chunks' entropy-coded bytes on the host; their upload and device decode run on the warps' stream, outside the warp events."""
+    chunks' entropy-coded bytes on the host; their upload and device decode run on the warps' stream, outside the warp events. A band
+    raster (geotiff.BandTiff) is uploaded raw and rendered to RGBA (rsb_tile_render, render_s) on the warps' stream before its warp."""
     import torch
 
     from robosat_b200.hostinfo import usable_cores
@@ -210,7 +219,7 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
     S, n = p.size, len(p.tiles)
     stats.update(step=p.step, mosaic_step=p.mosaic_step, candidates=p.candidates, warped=n, existing=0, predicted=0, batches=0,
                  windows=len(p.windows), image_slots=p.image_slots, plane_slots=p.plane_slots, store_bytes=p.store_bytes, decode_s=0.0,
-                 warp_s=0.0, predict_s=0.0, mosaic_s=0.0, sink_s=0.0)
+                 render_s=0.0, warp_s=0.0, predict_s=0.0, mosaic_s=0.0, sink_s=0.0)
     dev = torch.device(device)
     lib = _lib.load()
     plane, image = S * S, S * S * 3
@@ -219,21 +228,23 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
     exists = np.zeros(n, bool)
     main = torch.cuda.current_stream(dev)
     side = torch.cuda.Stream(device=dev)  # warps: their covered counts come back without waiting for the batches in flight
-    spp = raster.spp
+    bands = T.is_bands(raster)
     jpeg_host = T._jpeg_buffers(raster, p.warps, dev) if p.warps else None
     if p.warps:
-        src_bytes = max(w.rows * w.cols * spp for w in p.warps)
+        src_bytes = max(T.raw_bytes(raster, w.rows, w.cols) for w in p.warps)
         nmax = max(len(w.xs) for w in p.warps)
         if jpeg_host:
             src_host = jpeg_host["data"]
         else:
             src_host = [torch.empty((src_bytes,), dtype=torch.uint8, pin_memory=True) for _ in range(2)]
         src = torch.empty((src_bytes,), dtype=torch.uint8, device=dev)
+        if bands:
+            rgba = torch.empty((max(w.rows * w.cols * 4 for w in p.warps),), dtype=torch.uint8, device=dev)
         covered = torch.empty((nmax,), dtype=torch.int64, device=dev)
         misses = torch.zeros((2,), dtype=torch.int64, device=dev)
         counts_host = torch.empty((nmax + 2,), dtype=torch.int64, pin_memory=True)
     stitched = {}  # batch -> event recorded after its stitch (a later warp into the same image slots waits for it)
-    timing = {"warp_s": [], "predict_s": [], "mosaic_s": []}
+    timing = {"render_s": [], "warp_s": [], "predict_s": [], "mosaic_s": []}
 
     def timed(key):
         ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
@@ -268,7 +279,7 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
         stats["decode_s"] += pending_decode.result()
         nxt = decoder.submit(decode, k + 1) if k + 1 < len(p.warps) else None  # into the other pinned buffer, while this one warps
         with torch.cuda.stream(side):
-            nbytes = w.rows * w.cols * spp
+            nbytes = T.raw_bytes(raster, w.rows, w.cols)
             if jpeg_host:
                 keep = T._jpeg_decode(jpeg_host, k % 2, src[:nbytes])
             else:
@@ -279,6 +290,13 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
                 last = max((j for j in stitched if j <= p.wait[k]), default=None)
                 if last is not None:
                     side.wait_event(stitched[last])
+            pixels = src
+            if bands:
+                r0, r1 = timed("render_s")
+                r0.record(side)
+                T.render(lib, raster, src.data_ptr(), w.rows, w.cols, rgba.data_ptr())
+                r1.record(side)
+                pixels = rgba
             start, end = timed("warp_s")
             start.record(side)
             s0 = a % p.image_slots
@@ -286,7 +304,7 @@ def run(raster, p, predictor, resampling="bilinear", output="masks", nodata=0, s
             if parts[0][1] < b - a:  # the window wraps around the end of the ring: the rest goes to slot 0 on
                 parts.append((parts[0][1], b - a, 0))
             for q, (i0, i1, slot) in enumerate(parts):
-                T.warp(lib, resampling, src.data_ptr(), w, raster, nodes.data_ptr(), p.step, xy[i0:].data_ptr(), i1 - i0, S, images[slot].data_ptr(),
+                T.warp(lib, resampling, pixels.data_ptr(), w, raster, nodes.data_ptr(), p.step, xy[i0:].data_ptr(), i1 - i0, S, images[slot].data_ptr(),
                        image, covered[i0:].data_ptr(), misses[q:].data_ptr())
             end.record(side)
             counts_host[:b - a].copy_(covered[:b - a], non_blocking=True)

@@ -335,10 +335,22 @@ def is_jpeg(raster):
     return getattr(raster, "compression", None) == 7
 
 
+def is_bands(raster):
+    """whether `raster` is read under the band rule (geotiff.BandTiff): its windows are rendered to RGBA before the warp"""
+    return hasattr(raster, "bands")
+
+
+def raw_bytes(raster, rows, cols):
+    """bytes of a decoded window of rows x cols pixels: spp samples per pixel, or for a band raster k samples of bits / 8 bytes"""
+    return rows * cols * (raster.k * raster.sample_bytes if is_bands(raster) else raster.spp)
+
+
 def source_bytes(raster, box):
     """device bytes of a source window (row0, rows, col0, cols): its pixels, plus for a JPEG raster the staged bytes and the decoder
-    scratch of the chunks it touches (jpeg.extra_bytes)"""
-    n = box[1] * box[3] * raster.spp
+    scratch of the chunks it touches (jpeg.extra_bytes), and for a band raster its RGBA rendering"""
+    n = raw_bytes(raster, box[1], box[3])
+    if is_bands(raster):
+        n += box[1] * box[3] * 4
     if is_jpeg(raster):
         from robosat_b200 import jpeg
 
@@ -400,9 +412,26 @@ def entry_point(resampling):
     return "rsb_tile_average" if resampling == "average" else "rsb_tile_warp"
 
 
+def render(lib, raster, src, rows, cols, out):
+    """rsb_tile_render of a band raster's decoded window `src` (rows x cols pixels) into `out`, RGBA rows of 4 cols bytes (device
+    pointers), with the raster's scale, on the current stream"""
+    if raster.scale is None:
+        raise _lib.RsbError("%s: %d-bit samples need --scale or --stretch" % (raster.path, raster.bits))
+    scale = np.asarray(raster.scale, np.int32).reshape(-1)
+    _lib.check(lib.rsb_tile_render(src, rows, cols, raster.bits, len(raster.bands), int(raster.alpha), raster.nodata, scale.ctypes.data, out,
+                                   cols * 4, _lib.current_stream_ptr()), "rsb_tile_render")
+
+
+def warp_layout(raster):
+    """(spp, alpha, nodata) of the pixels the warp reads: the raster's own, or RGBA with alpha validity for a band raster"""
+    return (4, 1, -1) if is_bands(raster) else (raster.spp, int(raster.alpha), raster.nodata)
+
+
 def warp(lib, resampling, src, w, raster, nodes, step, tiles, n, size, out, image_stride, covered, misses):
-    """one launch of rsb_tile_warp or rsb_tile_average (device pointers) over Window `w`'s source and lattice, on the current stream"""
-    args = (src, w.cols * raster.spp, w.row0, w.col0, w.rows, w.cols, raster.width, raster.height, raster.spp, int(raster.alpha), raster.nodata,
+    """one launch of rsb_tile_warp or rsb_tile_average (device pointers) over Window `w`'s source (for a band raster, its RGBA
+    rendering) and lattice, on the current stream"""
+    spp, alpha, nodata = warp_layout(raster)
+    args = (src, w.cols * spp, w.row0, w.col0, w.rows, w.cols, raster.width, raster.height, spp, alpha, nodata,
             nodes, w.kx0, w.ky0, w.nodes.shape[1], w.nodes.shape[0], step, tiles, n, size)
     tail = (out, image_stride, covered, misses, _lib.current_stream_ptr())
     if resampling == "average":
@@ -422,8 +451,9 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
     """Warp the candidate tiles of `raster` (a GeoTiff), intersected with `tiles` (iterable of (x, y)) when given. For every window,
     sink(xy int64 [n, 2], images uint8 [n, size, size, 3], covered int64 [n]) is called on a writer thread with the tiles that have
     covered pixels (the arrays are reused after the call returns). Returns the int64 [n, 2] candidate tiles. `stats`, a dict,
-    receives the lattice step and seconds of decode, upload, warp (CUDA events) and sink. For a JPEG raster, decode is the staging of
-    the chunks' entropy-coded bytes on the host and upload includes their decode on the device."""
+    receives the lattice step and seconds of decode, upload, render and warp (CUDA events) and sink. For a JPEG raster, decode is the
+    staging of the chunks' entropy-coded bytes on the host and upload includes their decode on the device. A band raster
+    (geotiff.BandTiff) is decoded to its raw samples, uploaded, and rendered to RGBA by rsb_tile_render before the warp."""
     import torch
 
     if resampling not in RESAMPLINGS:
@@ -438,18 +468,19 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
     corner = resampling == "average"
     step = choose_step(raster, zoom, size, cand, corner)
     windows = plan(raster, zoom, size, cand, step, budget, batch, corner)
-    stats.update(step=step, candidates=len(cand), windows=len(windows), decode_s=0.0, upload_s=0.0, warp_s=0.0, sink_s=0.0, written=0)
+    stats.update(step=step, candidates=len(cand), windows=len(windows), decode_s=0.0, upload_s=0.0, render_s=0.0, warp_s=0.0, sink_s=0.0,
+                 written=0)
     if not windows:
         return cand
     from robosat_b200.cover import _alloc
 
     dev = torch.device(device)
-    spp = raster.spp
+    bands = is_bands(raster)
     jpeg_host = _jpeg_buffers(raster, windows, dev)
     if jpeg_host:
         src_host = jpeg_host["data"]
     else:
-        src_host = [_pinned(max(w.rows * w.cols * spp for w in windows)) for _ in range(2)]
+        src_host = [_pinned(max(raw_bytes(raster, w.rows, w.cols) for w in windows)) for _ in range(2)]
     nmax = max(len(w.xs) for w in windows)
     out_host = [_pinned(nmax * size * size * 3) for _ in range(2)]
     counts_host = [torch.empty((nmax,), dtype=torch.int64, pin_memory=True) for _ in range(2)]
@@ -480,6 +511,7 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
         return time.perf_counter() - t0, len(keep)
 
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    rendered = torch.cuda.Event(enable_timing=True)
     stream = torch.cuda.current_stream(dev)
     with ThreadPoolExecutor(1) as decoder, ThreadPoolExecutor(1) as writer:
         pending = decoder.submit(decode, 0)
@@ -491,7 +523,7 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
                     pending = decoder.submit(decode, k + 1)  # into the other pinned buffer, while this window is warped
                 n = len(w.xs)
                 t0 = time.perf_counter()
-                src = _alloc((w.rows * w.cols * spp,), torch.uint8, dev, "the %d x %d source window" % (w.cols, w.rows))
+                src = _alloc((raw_bytes(raster, w.rows, w.cols),), torch.uint8, dev, "the %d x %d source window" % (w.cols, w.rows))
                 if jpeg_host:
                     keep = _jpeg_decode(jpeg_host, k % 2, src)
                 else:
@@ -507,7 +539,12 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
                 covered = torch.empty((n,), dtype=torch.int64, device=dev)
                 misses = torch.empty((1,), dtype=torch.int64, device=dev)
                 start.record(stream)
-                warp(lib, resampling, src.data_ptr(), w, raster, nodes.data_ptr(), step, xy.data_ptr(), n, size, out.data_ptr(), size * size * 3,
+                pixels = src
+                if bands:
+                    pixels = _alloc((w.rows * w.cols * 4,), torch.uint8, dev, "the %d x %d RGBA window" % (w.cols, w.rows))
+                    render(lib, raster, src.data_ptr(), w.rows, w.cols, pixels.data_ptr())
+                rendered.record(stream)
+                warp(lib, resampling, pixels.data_ptr(), w, raster, nodes.data_ptr(), step, xy.data_ptr(), n, size, out.data_ptr(), size * size * 3,
                      covered.data_ptr(), misses.data_ptr())
                 end.record(stream)
                 if writes[k % 2] is not None:  # the writer is done with this buffer pair before it is overwritten
@@ -518,11 +555,12 @@ def run(raster, zoom, size, resampling="bilinear", tiles=None, sink=None, budget
                 counts_host[k % 2][:n].copy_(covered, non_blocking=True)
                 misses_host.copy_(misses, non_blocking=True)
                 torch.cuda.synchronize(dev)
-                stats["warp_s"] += start.elapsed_time(end) / 1e3
+                stats["render_s"] += start.elapsed_time(rendered) / 1e3
+                stats["warp_s"] += rendered.elapsed_time(end) / 1e3
                 if int(misses_host[0]):
                     raise _lib.RsbError("%s: %d samples of tiles %d..%d of row %d fell outside their source window (a planning error)" % (
                         entry_point(resampling), int(misses_host[0]), w.xs[0], w.xs[-1], w.y))
-                del src, out
+                del src, pixels, out
                 writes[k % 2] = writer.submit(deliver, k, n)
         finally:
             for f in writes:
@@ -573,3 +611,66 @@ def tile_device(raster, zoom, size, resampling="bilinear", tiles=None, budget=DE
 
     run(raster, zoom, size, resampling, tiles, sink, budget, batch, stats=stats)
     return got
+
+
+# ---- the band rule's contrast stretch ----
+
+DEFAULT_STATS_BUDGET = 256 << 20  # bytes of one row band of decoded samples (two pinned host copies, one device copy)
+
+
+def band_stats(raster, budget=DEFAULT_STATS_BUDGET, device="cuda", threads=None, stats=None):
+    """int64 [len(raster.bands), 2^bits]: the count of every value of each selected band over the valid pixels of the whole band
+    raster (geotiff.BandTiff), from rsb_band_histogram. The raster goes in full-width row bands of whole chunk rows under `budget`
+    bytes; each band is decoded on a host thread while the previous one is counted. `stats`, a dict, receives stats_s (seconds,
+    wall clock) and stats_bands (the row bands)."""
+    import torch
+
+    t0 = time.perf_counter()
+    dev = torch.device(device)
+    row_bytes = raw_bytes(raster, 1, raster.width)
+    step = max(1, budget // row_bytes // raster.chunk_h) * raster.chunk_h  # whole chunk rows: each chunk is decoded once
+    step = min(step, raster.height)
+    spans = [(r, min(step, raster.height - r)) for r in range(0, raster.height, step)]
+    host = [_pinned(step * row_bytes) for _ in range(min(2, len(spans)))]
+    src = torch.empty((step * row_bytes,), dtype=torch.uint8, device=dev)
+    hist = torch.zeros((len(raster.bands), 1 << raster.bits), dtype=torch.int64, device=dev)
+    lib = _lib.load()
+
+    def decode(i):
+        r0, rows = spans[i]
+        raster.read_window(r0, rows, 0, raster.width, out=host[i % 2].numpy(), threads=threads)
+
+    with ThreadPoolExecutor(1) as decoder:
+        pending = decoder.submit(decode, 0)
+        for i, (r0, rows) in enumerate(spans):
+            pending.result()
+            if i + 1 < len(spans):
+                pending = decoder.submit(decode, i + 1)  # into the other pinned buffer, while this band is counted
+            n = rows * row_bytes
+            src[:n].copy_(host[i % 2][:n], non_blocking=True)
+            _lib.check(lib.rsb_band_histogram(src.data_ptr(), rows, raster.width, raster.bits, len(raster.bands), int(raster.alpha), raster.nodata,
+                                              hist.data_ptr(), _lib.current_stream_ptr()), "rsb_band_histogram")
+            torch.cuda.synchronize(dev)  # the next decode into this pinned buffer waits for its upload
+    out = hist.cpu().numpy()
+    if stats is not None:
+        stats.update(stats_s=time.perf_counter() - t0, stats_bands=len(spans))
+    return out
+
+
+def stretch_scale(hist, q_lo, q_hi):
+    """[(LO, HI)] per band of `hist` (int64 [bands, values], band_stats) at the percentiles q_lo < q_hi given in hundredths of a
+    percent (0..10000): with N the band's count, rank = max(1, ceil(q N / 10000)), and the value is the smallest v whose cumulative
+    count reaches the rank. HI = LO gives HI = LO + 1 (LO = HI - 1 at the top value). RsbError when there is no valid pixel."""
+    hist = np.asarray(hist, np.int64)
+    top = hist.shape[1] - 1
+    pairs = []
+    for h in hist:
+        cum = np.cumsum(h)
+        n = int(cum[-1])
+        if n == 0:
+            raise _lib.RsbError("the raster has no valid pixel to stretch")
+        lo, hi = (int(np.searchsorted(cum, max(1, -(-q * n // 10000)), side="left")) for q in (int(q_lo), int(q_hi)))
+        if hi == lo:
+            lo, hi = (lo, lo + 1) if lo < top else (top - 1, top)
+        pairs.append((lo, hi))
+    return pairs

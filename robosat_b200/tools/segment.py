@@ -1,11 +1,14 @@
 """`rs segment`: an orthomosaic GeoTIFF in, one 1-band GeoTIFF of masks (or foreground probability bins) on the raster's own grid out.
 Its pixels are those of `rs tile → rs predict → rs masks → rs mosaic --like` run with the same settings (DESIGN.md §8), but the tiles,
 the network's bins and the masks never leave the GPU (`robosat_b200.segment`): no PNG is written or read. One device; RSB_GPUS is
-not read. An existing file is overwritten; a failed run leaves none. The reference has no such tool."""
+not read. An existing file is overwritten; a failed run leaves none. The reference has no such tool. --bands, --scale and --stretch read
+the raster under the band rule, as `rs tile` does."""
 
 import argparse
 import os
 import sys
+
+from robosat_b200.tools.tile import add_band_options
 
 
 def add_parser(subparser):
@@ -26,13 +29,15 @@ def add_parser(subparser):
     parser.add_argument("--model", type=str, required=True, help="path to model configuration file")
     parser.add_argument("--dataset", type=str, required=True, help="path to dataset configuration file")
     parser.add_argument("--checkpoint", type=str, required=True, help="model checkpoint to load")
+    add_band_options(parser)
     parser.add_argument("raster", type=str, help="path to the GeoTIFF")
     parser.add_argument("out", type=str, help="path of the GeoTIFF to write")
     parser.set_defaults(func=main)
 
 
 def main(args, stats=None, budget=None):
-    """`stats` (a dict), when given, receives segment.run's counts and seconds, the encode and write seconds and the total"""
+    """`stats` (a dict), when given, receives segment.run's counts and seconds, the --stretch pass's (stats_s), the encode and write
+    seconds and the total"""
     import time
 
     import torch
@@ -48,7 +53,7 @@ def main(args, stats=None, budget=None):
     from robosat_b200.hostinfo import usable_cores
     from robosat_b200.predictor import TilePredictor
     from robosat_b200.tools.predict import check_class_names, load_state_dict
-    from robosat_b200.tools.tile import read_tiles
+    from robosat_b200.tools.tile import apply_stretch, band_options, open_band_raster, read_tiles
 
     t0 = time.perf_counter()
     if not 0 <= args.zoom <= _lib.RSB_COVER_MAX_ZOOM:
@@ -75,15 +80,20 @@ def main(args, stats=None, budget=None):
             sys.exit("Error: dataset %s: %s" % (args.dataset, exc))
     if not load_config(args.model)["common"]["cuda"]:
         sys.exit("Error: robosat_b200 runs on CUDA devices only; set cuda = true in the model configuration")
+    opts = band_options(args)
     listed = read_tiles(args.tiles, args.zoom) if args.tiles else None
+    raster = open_band_raster(args.raster, opts) if opts else None
     if not torch.cuda.is_available():
         sys.exit("Error: CUDA requested but not available")
     _lib.require_device()
+    stats = stats if stats is not None else {}
     try:
-        raster = GeoTiff(args.raster)
+        raster = raster or GeoTiff(args.raster)
         grid = M.Grid(*read_grid(args.raster))
     except (_lib.RsbError, OSError) as e:
         sys.exit("Error: %s" % e)
+    if opts:
+        apply_stretch(raster, opts, stats, usable_cores())
     ratio = T.coarse_ratio(raster, args.zoom, args.size)
     if ratio > 2 and args.resampling != "average":
         print(T.W_COARSE.format(args.zoom, ratio), file=sys.stderr)
@@ -108,7 +118,6 @@ def main(args, stats=None, budget=None):
     predictor = TilePredictor(load_state_dict(args.checkpoint), len(classes), args.batch_size, args.size + 2 * args.overlap, overlap=args.overlap,
                               device=device, use_graph=os.environ.get("RSB_PREDICT_GRAPH", "1") == "1",
                               depth=int(os.environ.get("RSB_PREDICT_DEPTH", "3")), tta=args.tta)
-    stats = stats if stats is not None else {}
     threads = usable_cores()
     writer = M.TiffWriter(args.out, grid, SEG.output_palette(flat), args.nodata, level=PNG_LEVEL, threads=threads)
     try:
